@@ -1,7 +1,7 @@
 #!/usr/bin/env python
-"""bench.py -- LR event-frames/sec of the ESR hot path on B200 (BASELINE.json metric), one process per GPU.
+"""bench.py -- LR event-frames/sec of the ESR hot path on H100 (BASELINE.json metric), one process per GPU.
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--workload cfg2|cfg3|cfg4] [--impl ours|reference]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--workload cfg2|cfg3|cfg4] [--impl ours|reference] [--dump-outputs DIR]
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N ... bench.py --gpus N ...
 
 A "step" = one batch of B sequences x L LR event frames taken from raw events to redistributed SR events:
@@ -12,9 +12,13 @@ e2e     : the same step through the public API with pinned HOST buffers: H2D of 
           resulting event lists inside the timed region.
 parity  : one un-timed check per workload of the network output of the measured plan against the CPU oracle
           (all windows, carried state) -- `parity.rel_max` must stay below 1e-3 (north_star).
-roofline: FLOP-weighted achieved TFLOP/s of the dominant kernel FAMILY (every tcgen05 conv launch of one step, timed
-          live with CUDA events), against the measured sustained bf16 peak; `roofline_hbm` = the HBM-bound kernels
-          (count scatter, redistribution, small-channel full-resolution convs) against the measured copy bandwidth.
+roofline: FLOP-weighted achieved TFLOP/s of the dominant kernel FAMILY (every wgmma conv launch of one step, timed
+          live with CUDA events), against the bf16 peak; `roofline_hbm` = the HBM-bound kernels (count scatter,
+          redistribution, small-channel full-resolution convs) against the HBM bandwidth.  Both peaks are the measured ones
+          of MEASURED_PEAKS.json where that file exists, else the H100 SXM data sheet's (989 TFLOP/s dense bf16, 3.35 TB/s).
+dump    : --dump-outputs DIR writes what the last timed step returned -- the SR count tensor and the redistributed event
+          list -- as DIR/<name>.npy (float32; a fixed, seeded row sample where the 64 MB budget would be exceeded).  The
+          inputs are seeded, so two builds run with the same arguments can be compared output for output.
 configs : the other BASELINE.json network configurations (cfg3 4x SR; cfg4 4x SR long sequence) with their own
           value / e2e / parity / cpu_baseline; `sweep` = configs[4] (scatter + redistribute at 1e5..1e7 events).
 Multi-GPU: the path shards by batch with no data-path collective (inference); every rank runs the per-GPU batch of
@@ -171,23 +175,8 @@ def measured_peaks():
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
         d = json.load(open(p))
-        return d.get("bf16_tflops_sustained", 1443.7), d.get("hbm_gbs", 6574.1), "measured (MEASURED_PEAKS.json)"
-    return 1400.0, 6650.0, "fallback (B200_PROFILING.md)"
-
-
-def ncu_traffic(workload):
-    """dram__bytes_read.sum + dram__bytes_write.sum per launch of the dominant kernel, from the committed summary of an
-    `ncu --set full` capture (profiles/r2_ncu_traffic.json, written by tools/ncu_traffic.py with the capture's git hash).
-    Nothing is hard-coded here: no file, or no entry for this workload -> None."""
-    p = os.path.join(ROOT, "profiles", "r2_ncu_traffic.json")
-    try:
-        d = json.load(open(p))
-        e = d.get(workload)
-        if e:
-            return e
-    except Exception:
-        pass
-    return None
+        return d.get("bf16_tflops_sustained", 989.0), d.get("hbm_gbs", 3350.0), "measured (MEASURED_PEAKS.json)"
+    return 989.0, 3350.0, "H100 SXM data sheet (dense bf16, HBM3), not measured"
 
 
 # ------------------------------------------------------------------------------------------------------------------
@@ -501,30 +490,24 @@ def profile_launches(net, wl, dev, reps=5):
 def rooflines(rows, wl_name, peak_tf, peak_hbm, peak_src):
     """roofline (tensor, dominant family) + the HBM-bound small-channel convs from the per-launch table."""
     tc = [r for r in rows if r[1] == 0]
-    gru = [r for r in rows if r[1] == 3]
     direct = [r for r in rows if r[1] == 1]
     other = [r for r in rows if r[1] == 2]
     tot_ms = sum(r[2] for r in rows)
     fam_fl, fam_ms = sum(r[3] for r in tc), sum(r[2] for r in tc)
     fam_tf = fam_fl / (fam_ms * 1e-3) / 1e12 if fam_ms else 0.0
-    all_fl, all_ms = fam_fl + sum(r[3] for r in gru), fam_ms + sum(r[2] for r in gru)
-    all_tf = all_fl / (all_ms * 1e-3) / 1e12 if all_ms else 0.0
     best = max(tc, key=lambda r: r[3] / max(r[2], 1e-9), default=None)
     top = max(tc, key=lambda r: r[3], default=None)
     tf = lambda r: r[3] / (r[2] * 1e-3) / 1e12 if r and r[2] > 0 else 0.0
-    traffic = ncu_traffic(wl_name)
-    roof = {"kernel": "k_conv_tc / k_conv_tc_persist family (tcgen05 implicit-GEMM convs): every tensor-core conv launch of one step, FLOP-weighted",
+    roof = {"kernel": "k_conv_tc family (wgmma implicit-GEMM convs): every tensor-core conv launch of one step, FLOP-weighted",
             "bound": "tensor", "achieved": fam_tf, "peak": peak_tf, "unit": "TFLOP/s", "frac": fam_tf / peak_tf,
-            "peak_source": peak_src + ", bf16 sustained",
+            "peak_source": peak_src,
             "algorithmic_gflop_per_step": fam_fl / 1e9, "ms_per_step": fam_ms, "launches_per_step": len(tc),
             "share_of_step_kernel_time": fam_ms / tot_ms if tot_ms else None,
             "note": "algorithmic FLOPs (1x); the fp32-parity 3-pass split-bf16 product issues 3x that on the tensor pipe, so 1/3 is this family's ceiling",
-            "traffic": traffic["dram_bytes_per_launch"] if traffic else None, "traffic_source": traffic,
+            "traffic": None,
             "largest_launch": {"layer": top[0], "achieved": tf(top), "frac": tf(top) / peak_tf, "launch_ms": top[2],
                                "algorithmic_gflop": top[3] / 1e9} if top else None,
             "best_launch": {"layer": best[0], "achieved": tf(best), "frac": tf(best) / peak_tf, "launch_ms": best[2]} if best else None,
-            "with_gru_chain": {"achieved": all_tf, "frac": all_tf / peak_tf, "gru_chain_ms_per_step": sum(r[2] for r in gru),
-                               "gru_chain_tflops": tf(gru[0]) if gru else None},
             "per_layer": [{"layer": r[0], "ms": round(r[2], 5), "tflops": round(tf(r), 1)} for r in tc]}
     d_by, d_ms = sum(r[4] for r in direct), sum(r[2] for r in direct)
     small = {"kernel": "k_conv_mma<...> small-channel full-resolution convs (head+enc0, enc1, enc2, attention maps, recons[1,2], tail), byte-weighted",
@@ -537,6 +520,25 @@ def rooflines(rows, wl_name, peak_tf, peak_hbm, peak_src):
           "per_layer": [{"layer": r[0], "ms": round(r[2], 5), "GBps": round(r[4] / (r[2] * 1e-3) / 1e9, 1) if r[2] > 0 else None}
                         for r in other]}
     return roof, small, ew
+
+
+def dump_outputs(out_dir, arrays, budget=64 << 20):
+    """Writes each tensor as out_dir/<name>.npy (float32).  A tensor that does not fit in what is left of the budget is
+    reduced to a fixed, seeded sample of its rows along the last axis (<name>.npy) plus the sampled row indices
+    (<name>_rows.npy, float64), so that two runs sample the same rows."""
+    os.makedirs(out_dir, exist_ok=True)
+    left = budget
+    for name, t in arrays.items():
+        a = t.detach().to(torch.float32).cpu().numpy()
+        if a.nbytes > left:
+            rows = a.reshape(-1, a.shape[-1])
+            n = max(0, min(len(rows), left // (rows.shape[1] * 4 + 8)))
+            idx = np.sort(np.random.default_rng(0).choice(len(rows), n, replace=False))
+            np.save(os.path.join(out_dir, name + "_rows.npy"), idx.astype(np.float64))
+            a = rows[idx]
+            left -= idx.nbytes
+        np.save(os.path.join(out_dir, name + ".npy"), a)
+        left -= a.nbytes
 
 
 def run_workload(args, name, dev, rank, world, dist, steps, warmup, main):
@@ -559,7 +561,7 @@ def run_workload(args, name, dev, rank, world, dist, steps, warmup, main):
     xs, ys, ps, off = synth_events(B, L, lr, 100 + rank)
     h_xs, h_ys, h_ps, h_off = (t.pin_memory() for t in (xs, ys, ps, off))
     d_xs, d_ys, d_ps, d_off = (t.to(dev) for t in (xs, ys, ps, off))
-    flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)     # > 126 MB L2
+    flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)     # > 50 MB L2
 
     def barrier():
         if world > 1:
@@ -567,18 +569,18 @@ def run_workload(args, name, dev, rank, world, dist, steps, warmup, main):
         torch.cuda.synchronize()
 
     def timed(fn, k):
-        """per-step CUDA-event timing with an (untimed) L2 flush between steps; returns total ms"""
-        tot = 0.0
+        """per-step CUDA-event timing with an (untimed) L2 flush between steps; returns total ms and the last step's result"""
+        tot, out = 0.0, None
         for _ in range(k):
             flush.zero_()
             e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
             torch.cuda.synchronize()
             e0.record()
-            fn()
+            out = fn()
             e1.record()
             torch.cuda.synchronize()
             tot += e0.elapsed_time(e1)
-        return tot
+        return tot, out
 
     dev_step = lambda: pipe.run_device(d_xs, d_ys, d_ps, d_off, EVENTS_PER_FRAME)
     host_step = lambda: pipe.run_host(h_xs, h_ys, h_ps, h_off, EVENTS_PER_FRAME)
@@ -595,10 +597,12 @@ def run_workload(args, name, dev, rank, world, dist, steps, warmup, main):
         sampler.start()
     barrier()
     l0 = _lib.lib().esr_launch_count()
-    ms_dev = timed(dev_step, steps)
+    ms_dev, last = timed(dev_step, steps)
     launches = _lib.lib().esr_launch_count() - l0 + steps * pipe.graph_launches
+    if main and rank == 0 and args.dump_outputs:                      # before the next replay overwrites the graph's output buffers
+        dump_outputs(args.dump_outputs, {"sr_counts": last[0], "events": last[1]})
     barrier()
-    ms_e2e_sync = timed(host_step, steps) if main else 0.0            # one batch at a time (latency view)
+    ms_e2e_sync = timed(host_step, steps)[0] if main else 0.0         # one batch at a time (latency view)
     barrier()
 
     # throughput view of the same end-to-end path: submit(i+1) is issued before finish(i), so the GPU runs batch i+1's network while
@@ -827,6 +831,8 @@ def main():
     ap.add_argument("--no-train", action="store_true", help="skip the training-iteration measurement (the `train` key)")
     ap.add_argument("--no-parity", action="store_true", help="skip the un-timed oracle check of the measured plan")
     ap.add_argument("--no-extra", action="store_true", help="skip the other configs (cfg3 / cfg4) and the cfg5 sweep")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="write the outputs of the last timed step (SR counts, event list) as DIR/<name>.npy, 64 MB at most")
     args = ap.parse_args()
     # stdout carries exactly ONE line (the JSON): anything a library prints there (NCCL's version banner at N > 1) goes to stderr
     sys.stdout.flush()
@@ -841,6 +847,8 @@ def main():
     args.warmup = max(args.warmup, 3) if args.impl == "ours" else args.warmup
 
     if args.impl == "reference":
+        if args.dump_outputs:
+            ap.error("--dump-outputs writes what the GPU path computed; it does not apply to --impl reference")
         run_reference(args, wl, rank, world)
         return
 
@@ -893,7 +901,7 @@ def main():
         res.pop("_ew", None)
         if args.profile_out:
             with open(args.profile_out, "w") as f:
-                f.write("idx,layer,class(0=tc,1=small-channel conv,2=other,3=gru_chain),ms,algorithmic_flops,algorithmic_bytes\n")
+                f.write("idx,layer,class(0=tc,1=small-channel conv,2=other),ms,algorithmic_flops,algorithmic_bytes\n")
                 for i, r in enumerate(rows):
                     f.write("%d,%s,%d,%.5f,%.0f,%.0f\n" % (i, r[0], r[1], r[2], r[3], r[4]))
         line = {"metric": "LR event-frames/sec", "value": res["value"], "unit": "frames/s", "n_gpus": world, "steps": args.steps,

@@ -1,5 +1,5 @@
 """Drop-in for the reference's `dataloader.cython_cnt2event.cnt2event` Cython module and its
-`cnt2event_api` wrapper, backed by the sm_100a kernels.
+`cnt2event_api` wrapper, backed by the sm_90a kernels.
 
   cnt2event(event_cnt: np.ndarray[float32, ndim=4], mode: int) -> np.ndarray[float32, (B, maxlen, 4)]
         same signature / dtype checks as cnt2event.pyx:18-19

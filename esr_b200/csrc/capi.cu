@@ -26,7 +26,7 @@ void set_error(const char *fmt, ...)
 const DevInfo &dev_info()
 {
     static DevInfo info = [] {
-        DevInfo d{148, 232448};
+        DevInfo d{132, 232448};
         int dev = 0;
         if (cudaGetDevice(&dev) == cudaSuccess) {
             cudaDeviceGetAttribute(&d.sm_count, cudaDevAttrMultiProcessorCount, dev);

@@ -1,4 +1,4 @@
-// common.cuh -- shared host/device helpers of libesr_b200 (sm_100a only).
+// common.cuh -- shared host/device helpers of libesr_b200 (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <cuda_bf16.h>
@@ -44,7 +44,7 @@ inline void count_launch(int n = 1) { g_launches.fetch_add(n, std::memory_order_
 
 // ---------------------------------------------------------------------------------------------
 // Programmatic dependent launch (PDL).  The network is ~50 dependent kernels of 20-200 us; a normal stream edge drains the GPU
-// between two of them (tail of the last wave, launch latency, the next kernel's prologue: barrier init, TMEM allocation,
+// between two of them (tail of the last wave, launch latency, the next kernel's prologue: barrier init,
 // descriptor fetch).  With the programmatic-serialization attribute the next grid is launched as soon as every CTA of the
 // current one has executed `griddepcontrol.launch_dependents` (first instruction of our kernels): its CTAs take over SMs as
 // they free up and run their prologue, then block in `griddepcontrol.wait` until the predecessor grid has COMPLETED and its
@@ -83,7 +83,7 @@ const DevInfo &dev_info();
 
 // ---------------------------------------------------------------------------------------------
 // split-bf16 activation storage: value = float(hi) + float(lo).  hi = RN_bf16(v), lo = RN_bf16(v - hi).
-// The two planes are what the tcgen05 kernels consume directly as MMA operands (3-pass product
+// The two planes are what the wgmma kernels consume directly as MMA operands (3-pass product
 // hi*hi + lo*hi + hi*lo, fp32 accumulate), giving ~2^-17 relative operand error.
 // ---------------------------------------------------------------------------------------------
 #ifdef __CUDACC__

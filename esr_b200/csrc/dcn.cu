@@ -4,10 +4,10 @@
 // sample at (y-1+i+off_h, x-1+j+off_w) only if it lies in (-1, H) x (-1, W); columns = value * mask).
 // Stride 1, pad 1, dilation 1, 3x3, 64 channels, 8 deformable groups of 8 channels (models/model.py:173).
 //
-// Layout choices for the B200: features are split-bf16 NHWC so the 8 channels of one group at one corner are one
+// Layout choices: features are split-bf16 NHWC so the 8 channels of one group at one corner are one
 // 16-byte load per plane; one thread = one (pixel, tap, group); its 8 outputs land at column tap*64 + g*8, i.e. eight
 // consecutive threads (g = 0..7) write one contiguous 128-byte row segment.  The columns tensor is then consumed by the
-// tcgen05 GEMM (tc_conv.cu, 1x1 mode over 9 K-chunks) with the DCN weight packed tap-major, which equals the
+// wgmma GEMM (tc_conv.cu, 1x1 mode over 9 K-chunks) with the DCN weight packed tap-major, which equals the
 // reference's W[Co, Ci*9] . columns contraction (dcn_v2_cuda.cu:90-92).
 #include "net.cuh"
 

@@ -1,8 +1,8 @@
 // dcn_bwd.cu -- backward of the modulated deformable 3x3 convolution (the `_ext.dcn_v2_backward` operator).
 // Reference: models/DCNv2/src/cuda/dcn_v2_cuda.cu:97-216 (per-sample loop: W^T.gO, col2im, coord kernel, gO.cols^T, gO.1)
 // with kernels models/DCNv2/src/cuda/dcn_v2_im2col_cuda.cu:197-254 (col2im, atomicAdd) and :256-327 (offset / mask grads).
-// Same analytic gradients, organised for the B200 data layout:
-//   1. gcols[p][tap*64+c] = sum_co gO[p][co] * W[co][c][tap]     tcgen05 GEMM (tc_conv.cu, 1x1 mode, 3 launches of N=192)
+// Same analytic gradients, organised for the split-bf16 NHWC data layout:
+//   1. gcols[p][tap*64+c] = sum_co gO[p][co] * W[co][c][tap]     wgmma GEMM (tc_conv.cu, 1x1 mode, 3 launches of N=192)
 //   2. one thread per (pixel, tap, group) re-derives the bilinear corners and, for its 8 channels,
 //        grad_mask   += gcols * sample                      grad_offset += gcols * mask * d(sample)/d(h,w)
 //        grad_input  += corner weight * gcols * mask        (fp32 atomicAdd, like the reference's col2im)

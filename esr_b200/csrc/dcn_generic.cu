@@ -1,6 +1,6 @@
 // dcn_generic.cu -- the `_ext.dcn_v2_forward` / `_ext.dcn_v2_backward` operators for ANY configuration the reference's
 // operator accepts (channels, groups, kernel size, stride, padding, dilation): the shapes other than the one ESR's network
-// uses (64 -> 64, 3x3, 8 groups, which runs on the tcgen05 path of dcn.cu / dcn_fused.cu / dcn_bwd.cu).  The reference's own
+// uses (64 -> 64, 3x3, 8 groups, which runs on the wgmma path of dcn.cu / dcn_fused.cu / dcn_bwd.cu).  The reference's own
 // tests and examples call the operator with 2 -> 2 channels on 4x4 maps and with deformable_groups = 2
 // (models/DCNv2/testcuda.py:14-17, 169-180), so a drop-in has to serve them.
 //

@@ -18,8 +18,8 @@ namespace esr {
 
 // Output tile geometry.  Tiled layers: a thread owns TPW x 2 pixels x C channels, C = 16 (COUT=64) or 8; the COUT/C
 // channel groups are spread over warps, so narrower layers get wider tiles (more pixels per block, 16-byte stores
-// everywhere).  TPW = 4 (more weight reuse per thread) is implemented but measured SLOWER on B200 for enc1 / recons[1,2]
-// (fewer resident blocks per SM), so every layer currently uses TPW = 2.
+// everywhere).  TPW = 4 (more weight reuse per thread) is implemented; every layer currently uses TPW = 2 (more resident
+// blocks per SM).
 template <int COUT, int TPW> struct DcGeom {
     static constexpr bool TILED = COUT >= 8;
     static constexpr int C = COUT >= 64 ? 16 : (COUT >= 8 ? 8 : COUT);

@@ -1,4 +1,4 @@
-// events.cu -- the integer/byte side of the hot path on sm_100a:
+// events.cu -- the integer/byte side of the hot path on sm_90a:
 //   events -> polarity count images (atomic scatter), dense counts / stacks -> time-sorted event lists
 //   (round-half-even -> exclusive scan -> expand -> stable LSD radix sort on (sample, t) -> padded rows).
 // Reference behaviour restated from dataloader/encodings.py:243-304, dataloader/h5dataset.py:508-528,

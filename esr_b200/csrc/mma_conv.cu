@@ -2,14 +2,14 @@
 // path (mma.sync m16n8k16 / m16n8k8, bf16 operands, fp32 accumulate) instead of FFMA loops.
 //
 // These layers (head+encoder 8->16->32->64 stride 2, decoder bilinear x2 + conv 32->16->8, tail 8->2;
-// models/model.py:20-45, 264-291, 309) have too few channels for a 128 x N tcgen05 tile and their inputs are produced on
+// models/model.py:20-45, 264-291, 309) have too few channels for a 128 x N wgmma tile and their inputs are produced on
 // the fly (fused head, fused bilinear upsampling), which TMA cannot do -- so the operand tile is built by the CTA itself:
 //   stage 1  the input patch of the output tile (+1 halo) is written to shared memory as split bf16 (hi and lo planes),
 //            pixel-major [py][px][CIN] with a 16-byte pad per pixel (conflict-free ldmatrix rows); the split source is
 //            copied as is, the decoder's bilinear x2 and the fused head conv are evaluated in fp32 and split here;
 //   stage 2  implicit GEMM per warp: A fragments (16 consecutive output pixels x 16 channels of one tap) by ldmatrix
 //            straight from the patch (lane addresses carry the stride and the tap shift), B fragments (weights, split,
-//            [tap][co][ci]) by 32-bit shared loads, three MMAs per K step (lo*hi + hi*lo + hi*hi) like the tcgen05 path;
+//            [tap][co][ci]) by 32-bit shared loads, three MMAs per K step (lo*hi + hi*lo + hi*hi) like the wgmma path;
 //   stage 3  accumulators -> shared memory (fp32) -> bias/activation already applied -> 16-byte split-bf16 stores (or the
 //            cropped fp32 NCHW output of the tail).
 // Same DirectArgs interface and results within the split-bf16 operand error (2^-17) of the fp32 kernels in direct_conv.cu,
@@ -455,11 +455,7 @@ int pack_mma_weight_dx(const float *w, int layer_cout, int layer_cin, void *dst,
     return ESR_OK;
 }
 
-// returns ESR_EINVAL for kinds that stay on the FFMA kernels.  Measured on B200 (cfg2, profiles/r1_notes.md), FFMA -> mma.sync:
-// enc1 88 -> 48, enc2 97 -> 43, recons[1] 203 -> 98, recons[2] 230 -> 146, tail 103 -> 64, attention maps 37 -> 23 and 62 -> 37 us
-// (with the unpack-once upsampling fill and the conflict-free unpadded 16- / 32-byte pixel layouts);
-// fused head+enc0 173 (FFMA) -> 174 (FFMA head + mma encoder, 4-way ldmatrix conflicts) -> ~123 (SWZ8 layout) -> see
-// profiles/r1_notes.md for the version with the head itself on mma.sync.
+// returns ESR_EINVAL for kinds that stay on the FFMA kernels
 int conv_mma(DirectKind kind, const DirectArgs &a, cudaStream_t st)
 {
     if (!a.w_mma) return ESR_EINVAL;

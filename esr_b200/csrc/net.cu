@@ -1,4 +1,4 @@
-// net.cu -- DeepRecurrNet.forward (models/model.py:294-344) as a fixed launch sequence over the sm_100a kernels.
+// net.cu -- DeepRecurrNet.forward (models/model.py:294-344) as a fixed launch sequence over the sm_90a kernels.
 //
 // A "net" is a plan for one (B, N=3, H, W): every intermediate tensor has a fixed place in a caller-provided
 // workspace, every TMA tensor map / launch descriptor is built once at creation, and forward() only enqueues
@@ -106,9 +106,8 @@ struct Net {
     ConvTCArgs c_pm0, c_pm1, c_lf1, c_lf2, c_lf3, c_gx, c_gf, c_of0, c_of1, c_com, c_dcn, c_cb0, c_cb1, c_ker, c_df0, c_df1,
         c_dn0, c_dn1, c_at0, c_rc0;
     std::vector<ConvTCArgs> c_gzr, c_go;
+    void *gru_plan = nullptr;          // the ConvGRU recurrence as one cooperative launch (opt-in); nullptr = two launches per step
     void *dcn_plan = nullptr;          // fused sampling + contraction (dcn_fused.cu); nullptr = columns + 1x1 GEMM
-    void *gru_plan = nullptr;          // cooperative whole-chain kernel (gru_chain.cu); nullptr = per-step launches
-    unsigned int *gru_barrier = nullptr;
     DirectArgs d[D_COUNT];
     bool agg_fused = false;            // scale aggregation of decoder levels 1, 2 inside the recons convs' fill
 };
@@ -182,7 +181,6 @@ static size_t layout(Net &n)
     n.m_gf_f = ints(VN); n.m_gf_r = ints(VN); n.m_gfres = ints(VN);
     n.m_gx.resize(nsteps); n.m_gh.resize(nsteps);
     for (int s = 0; s < nsteps; ++s) { n.m_gx[s] = ints(2 * B); n.m_gh[s] = ints(2 * B); }
-    n.gru_barrier = (unsigned int *)A.take(64 * 8 * sizeof(unsigned int));   // per-image phase counters of the GRU chain kernel
     return A.off;
 }
 
@@ -303,13 +301,10 @@ static int build(Net &n, cudaStream_t st)
         d.epi_mode = EPI_GRU_OUT; d.h_prev = view_imgs(n.hs, g * 2 * B); d.z_buf = n.zbuf; d.out = view_imgs(n.hs, (g + 1) * 2 * B);
         if ((rc = conv_tc_prepare(d, &n.c_go[g]))) return rc;
     }
-    // the same chain as ONE cooperative kernel (default); ESR_GRU_PER_STEP=1 keeps the two-launches-per-step path
-    static const bool per_step = getenv("ESR_GRU_PER_STEP") != nullptr;
-    if (!per_step) {
-        if ((rc = gru_chain_prepare(n.xc, n.hs, n.rh, n.zbuf, pw(n, T_GZR), pb(n, T_GZR), pw(n, T_GO), pb(n, T_GO), n.gru_barrier,
-                                    B, N, nsteps, &n.gru_plan)))
-            return rc;
-    }
+    // ESR_GRU_CHAIN=1: the whole chain as ONE cooperative kernel (bit-identical).  Opt-in: on H100 it measured no faster than two
+    // launches per step (cfg2: 6.61 / 6.68 vs 6.58 / 6.43 ms per step, alternating, DESIGN.md 8c) -- one 168-register CTA per SM and
+    // 36 grid barriers against PDL-overlapped launches with two CTAs per SM on the N = 64 phase.  Read per net, so a test can build both.
+    if (getenv("ESR_GRU_CHAIN") != nullptr && (rc = gru_chain_prepare(n.c_gzr, n.c_go, &n.gru_plan))) return rc;
     d = mk(n, T_GF, VN, ACT_RELU); d.n_src = 2; d.src[0] = n.hs; d.src_img[0] = n.m_gf_f; d.src[1] = n.hs; d.src_img[1] = n.m_gf_r;
     d.res_mode = RES_POST_ACT; d.res = n.F; d.res_img = n.m_gfres; d.out = n.tp;
     if ((rc = conv_tc_prepare(d, &n.c_gf))) return rc;
@@ -392,7 +387,7 @@ struct Prof {
     struct Entry { cudaEvent_t e0, e1; int cls; double flops, bytes; const char *name; };
     std::vector<Entry> entries;
 };
-enum ProfClass : int { PC_TC = 0, PC_DIRECT = 1, PC_OTHER = 2, PC_GRU = 3 };
+enum ProfClass : int { PC_TC = 0, PC_DIRECT = 1, PC_OTHER = 2 };
 
 static double tc_flops(const ConvTCArgs &a) { return 2.0 * a.n_img * a.H * a.W * (double)a.cout * (double)a.nkb * 64.0; }
 static double direct_flops(int dl, const DirectArgs &a)
@@ -470,7 +465,7 @@ static int forward(Net &n, const float *input, const int *in_img, float *output,
     if (n.gru_plan) {
         double fl = 0.0, by = 0.0;
         for (int g = 0; g < nsteps; ++g) { fl += tc_flops(n.c_gzr[g]) + tc_flops(n.c_go[g]); by += tc_bytes(n.c_gzr[g]) + tc_bytes(n.c_go[g]); }
-        RUNC("gru.chain", PC_GRU, fl, by, gru_chain_launch(n.gru_plan, st));
+        RUNC("gru.chain", PC_TC, fl, by, gru_chain_launch(n.gru_plan, st));
     } else {
         for (int g = 0; g < nsteps; ++g) {
             RUNT("gru.zr", n.c_gzr[g]);
@@ -604,8 +599,8 @@ extern "C" int esr_net_create(esr_net_t *out, int B, int N, int L, int H, int W,
 
 extern "C" int esr_net_destroy(esr_net_t net)
 {
-    if (net && ((Net *)net)->gru_plan) gru_chain_destroy(((Net *)net)->gru_plan);
     if (net && ((Net *)net)->dcn_plan) dcn_fused_destroy(((Net *)net)->dcn_plan);
+    if (net && ((Net *)net)->gru_plan) gru_chain_destroy(((Net *)net)->gru_plan);
     delete (Net *)net;
     return ESR_OK;
 }

@@ -74,18 +74,11 @@ int conv_narrow_tail(const SplitTensor &x, const float *w, const float *bias, in
 int dcn_columns(const SplitTensor &feat, const int *feat_img, const float *om, int n_img, const SplitTensor &cols /*C=576*/,
                 cudaStream_t st);
 
-// ---- DCNv2 with the sampling fused into the tcgen05 contraction (dcn_fused.cu): no columns tensor in HBM
+// ---- DCNv2 with the sampling fused into the wgmma contraction (dcn_fused.cu): no columns tensor in HBM
 int dcn_fused_prepare(const SplitTensor &feat, const int *feat_img, const float *om, const void *wpacked, const float *bias,
                       int n_img, int act, const SplitTensor &out, void **plan_out);
 int dcn_fused_launch(void *plan, cudaStream_t st);
 void dcn_fused_destroy(void *plan);
-
-// ---- the ConvGRU recurrence of a whole sequence batch in one cooperative kernel (gru_chain.cu)
-int gru_chain_prepare(const SplitTensor &xc, const SplitTensor &hs, const SplitTensor &rh, float *zbuf, const void *w_zr,
-                      const float *b_zr, const void *w_go, const float *b_go, unsigned int *barrier, int B, int N,
-                      int nsteps, void **plan_out);
-int gru_chain_launch(void *plan, cudaStream_t st);
-void gru_chain_destroy(void *plan);
 
 // ---- the operators for any other configuration (dcn_generic.cu): fp32 CUDA-core kernels, reference NCHW layouts
 size_t dcn_generic_ws_bytes(int B, int C, int H, int W, int Co, int kernel, int stride, int pad, int dil, int G, int backward);

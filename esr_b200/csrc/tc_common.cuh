@@ -1,23 +1,22 @@
-// tc_common.cuh -- device-side building blocks shared by the tcgen05 convolution kernels (tc_conv.cu, tc_conv3.cu):
-// PTX wrappers (mbarrier, TMA, tcgen05 alloc/mma/commit/ld), UMMA descriptors, split-bf16 vector I/O and the fused epilogue.
+// tc_common.cuh -- device-side building blocks shared by the Hopper tensor-core kernels (tc_conv.cu, dcn_fused.cu, wgrad_tc.cu):
+// PTX wrappers (mbarrier, TMA, wgmma), shared-memory matrix descriptors, the accumulator staging of the epilogues, split-bf16 vector
+// I/O and the fused conv epilogue.
 #pragma once
 #include "tc_conv.cuh"
 
 namespace esr {
 
-constexpr int TC_THREADS = 192;
-constexpr int TC_BLOCK_M = 128;
+constexpr int TC_BLOCK_M = 128;                       // output pixels per tile: two warpgroups x 64 rows
 constexpr int TC_A_BYTES = TC_BLOCK_M * 128;          // one plane of one A tile: 128 rows x 64 bf16
+constexpr int TC_STG_LD = 68;                         // row stride (floats) of an epilogue staging tile: 64 columns + 4 (bank spread)
+constexpr uint32_t TC_STG_BYTES = 64u * TC_STG_LD * 4u; // one warpgroup's staging tile: 64 rows x 64 fp32 columns
 
 // ------------------------------------------------------------------------------------------------
 // PTX wrappers
 // ------------------------------------------------------------------------------------------------
 __device__ __forceinline__ uint32_t smem_u32(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }
 
-// One lane of a CONVERGED warp.  Unlike `lane == 0`, elect.sync tells ptxas that exactly one thread runs the guarded code, so the
-// uniform-datapath instructions inside (UTCHMMA, UTMALDG, UTCBAR) are emitted directly instead of each being wrapped in an
-// ELECT / BRA.U.ANY loop over the "possibly many" active lanes -- measured on B200: 69-74 cycles per tcgen05.mma issued from an
-// `if (lane == 0)` block, which made the N <= 64 layers issue-bound (profiles/r2_notes.md).
+// One lane of a CONVERGED warp (the single-thread TMA issuers).
 __device__ __forceinline__ bool elect_one_sync()
 {
     uint32_t pred;
@@ -30,39 +29,6 @@ __device__ __forceinline__ bool elect_one_sync()
     return pred != 0;
 }
 
-// ---- thread-block cluster helpers (CTA pairs of tc_conv.cu, per-image clusters of gru_chain.cu)
-__device__ __forceinline__ uint32_t pair_rank()
-{
-    uint32_t r;
-    asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-    return r;
-}
-__device__ __forceinline__ void pair_sync()
-{
-    asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-// arrive on the barrier at the same shared-memory offset in CTA `cta` of the cluster
-__device__ __forceinline__ void mbar_arrive_remote(uint32_t bar, uint32_t cta)
-{
-    asm volatile(
-        "{\n\t"
-        ".reg .b32 raddr;\n\t"
-        "mapa.shared::cluster.u32 raddr, %0, %1;\n\t"
-        "mbarrier.arrive.release.cluster.shared::cluster.b64 _, [raddr];\n\t"
-        "}" ::"r"(bar), "r"(cta) : "memory");
-}
-__device__ __forceinline__ void mbar_wait_cluster(uint32_t bar, uint32_t parity)
-{
-    uint32_t done;
-    do {
-        asm volatile(
-            "{\n\t"
-            ".reg .pred P1;\n\t"
-            "mbarrier.try_wait.parity.acquire.cluster.shared::cta.b64 P1, [%1], %2;\n\t"
-            "selp.u32 %0, 1, 0, P1;\n\t"
-            "}" : "=r"(done) : "r"(bar), "r"(parity) : "memory");
-    } while (!done);
-}
 __device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count)
 {
     asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(count) : "memory");
@@ -70,6 +36,10 @@ __device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count)
 __device__ __forceinline__ void mbar_expect_tx(uint32_t bar, uint32_t bytes)
 {
     asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
+}
+__device__ __forceinline__ void mbar_arrive(uint32_t bar)
+{
+    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
 }
 __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity)
 {
@@ -83,8 +53,8 @@ __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity)
         "DONE:\n\t"
         "}" ::"r"(bar), "r"(parity) : "memory");
 }
-// same, for waits that last microseconds (an MMA / producer thread idling while other warps of the CTA do the real work): back
-// off between polls so the spin does not eat the issue slots of the warps it is waiting for
+// same, for waits that last microseconds (a producer thread idling while other warps of the CTA do the real work): back off
+// between polls so the spin does not eat the issue slots of the warps it is waiting for
 __device__ __forceinline__ void mbar_wait_backoff(uint32_t bar, uint32_t parity)
 {
     uint32_t done;
@@ -111,94 +81,158 @@ __device__ __forceinline__ void tma_load_3d(const CUtensorMap *map, uint32_t bar
                  " [%0], [%1, {%3, %4, %5}], [%2];"
                  ::"r"(dst), "l"(map), "r"(bar), "r"(c0), "r"(c1), "r"(c2) : "memory");
 }
-__device__ __forceinline__ void tmem_alloc(uint32_t dst_smem, uint32_t cols)
+// named barrier over `count` threads (id 0 is __syncthreads)
+__device__ __forceinline__ void named_sync(int id, int count)
 {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(dst_smem), "r"(cols) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
+    asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(count) : "memory");
 }
-__device__ __forceinline__ void tmem_dealloc(uint32_t addr, uint32_t cols)
-{
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(addr), "r"(cols) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
 
-// D[tmem] (+)= A[smem desc] * B[smem desc]^T, bf16 x bf16 -> fp32
-__device__ __forceinline__ void umma_bf16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accum)
+// ------------------------------------------------------------------------------------------------
+// wgmma (sm_90a): D[64 rows, N] (+)= A[64 x 16, smem] * B[16 x N, smem], bf16 x bf16 -> fp32 registers of one warpgroup.
+// Accumulator fragment of thread (warp w of the warpgroup, lane l), register i:
+//   row = 16 w + l / 4 + 8 ((i / 2) % 2),   column = 8 (i / 4) + 2 (l % 4) + i % 2
+// ------------------------------------------------------------------------------------------------
+// 128B-swizzled operand tile: rows of 128 bytes, 8-row groups 1024 bytes apart (SBO).  K-major: LBO unused.  MN-major: LBO =
+// distance between 64-element column blocks.  Bits: start>>4 [0,14) | LBO>>4 [16,30) | SBO>>4 [32,46) | SWIZZLE_128B (1) [62,64).
+// Advancing the operand by n bytes (n a multiple of 16, the result below 256 KB) is desc + n / 16.
+__device__ __forceinline__ uint64_t wgmma_desc(uint32_t smem_addr, uint32_t lbo_bytes = 16u)
+{
+    return (uint64_t)((smem_addr & 0x3FFFFu) >> 4) | ((uint64_t)((lbo_bytes >> 4) & 0x3FFFu) << 16) |
+           ((uint64_t)(1024u >> 4) << 32) | ((uint64_t)1 << 62);
+}
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N> __device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// keeps the compiler from moving accumulator reads / writes across the asynchronous MMAs
+template <int R> __device__ __forceinline__ void acc_fence(float *acc)
+{
+#pragma unroll
+    for (int i = 0; i < R; ++i) asm volatile("" : "+f"(acc[i])::"memory");
+}
+
+// TNSP = 0: both operands K-major; 1: both MN-major
+template <int TNSP> __device__ __forceinline__ void wgmma_n16(float *d, uint64_t da, uint64_t db)
 {
     asm volatile(
-        "{\n\t"
-        ".reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t"
-        "}" ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accum) : "memory");
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n16k16.f32.bf16.bf16 {"
+        "%0, %1, %2, %3, %4, %5, %6, %7}, %8, %9, p, 1, 1, %10, %10;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+        : "l"(da), "l"(db), "n"(TNSP));
 }
-__device__ __forceinline__ void umma_commit(uint32_t bar)
+template <int TNSP> __device__ __forceinline__ void wgmma_n32(float *d, uint64_t da, uint64_t db)
 {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n32k16.f32.bf16.bf16 {"
+        "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, p, 1, 1, %18, %18;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+          "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+        : "l"(da), "l"(db), "n"(TNSP));
 }
-__device__ __forceinline__ void tmem_ld32(uint32_t addr, uint32_t (&v)[32])
+template <int TNSP> __device__ __forceinline__ void wgmma_n64(float *d, uint64_t da, uint64_t db)
 {
-    asm volatile("tcgen05.ld.sync.aligned.32x32b.x32.b32"
-                 "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15,"
-                 " %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-                 : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]),
-                   "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]),
-                   "=r"(v[16]), "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]),
-                   "=r"(v[24]), "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-                 : "r"(addr));
-    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 {"
+        "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15,"
+        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1, %34, %34;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+          "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+          "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+          "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+        : "l"(da), "l"(db), "n"(TNSP));
+}
+template <int TNSP> __device__ __forceinline__ void wgmma_n128(float *d, uint64_t da, uint64_t db)
+{
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 {"
+        "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15,"
+        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31,"
+        "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47,"
+        "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1, %66, %66;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+          "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+          "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+          "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+          "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+          "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+          "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+          "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+        : "l"(da), "l"(db), "n"(TNSP));
+}
+template <int TNSP> __device__ __forceinline__ void wgmma_n256(float *d, uint64_t da, uint64_t db)
+{
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n256k16.f32.bf16.bf16 {"
+        "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15,"
+        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31,"
+        "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47,"
+        "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63,"
+        "%64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79,"
+        "%80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95,"
+        "%96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111,"
+        "%112, %113, %114, %115, %116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127}, %128, %129, p, 1, 1, %130, %130;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+          "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+          "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+          "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+          "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+          "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+          "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+          "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]),
+          "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]),
+          "+f"(d[72]), "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79]),
+          "+f"(d[80]), "+f"(d[81]), "+f"(d[82]), "+f"(d[83]), "+f"(d[84]), "+f"(d[85]), "+f"(d[86]), "+f"(d[87]),
+          "+f"(d[88]), "+f"(d[89]), "+f"(d[90]), "+f"(d[91]), "+f"(d[92]), "+f"(d[93]), "+f"(d[94]), "+f"(d[95]),
+          "+f"(d[96]), "+f"(d[97]), "+f"(d[98]), "+f"(d[99]), "+f"(d[100]), "+f"(d[101]), "+f"(d[102]), "+f"(d[103]),
+          "+f"(d[104]), "+f"(d[105]), "+f"(d[106]), "+f"(d[107]), "+f"(d[108]), "+f"(d[109]), "+f"(d[110]), "+f"(d[111]),
+          "+f"(d[112]), "+f"(d[113]), "+f"(d[114]), "+f"(d[115]), "+f"(d[116]), "+f"(d[117]), "+f"(d[118]), "+f"(d[119]),
+          "+f"(d[120]), "+f"(d[121]), "+f"(d[122]), "+f"(d[123]), "+f"(d[124]), "+f"(d[125]), "+f"(d[126]), "+f"(d[127])
+        : "l"(da), "l"(db), "n"(TNSP));
 }
 
-// one epilogue chunk of accumulator columns [n0, n0 + 32) (16 valid columns when fewer remain: npad is a multiple of 16)
-__device__ __forceinline__ void tmem_ld_chunk(uint32_t taddr, int n0, int npad, uint32_t (&raw)[32])
+// D[64, NP] (+)= A * B for any NP that is a multiple of 16 up to 256: one instruction per set bit of NP (the fragment layout above
+// makes the concatenated accumulators one [NP / 2] array).  The B operand of columns [c, ...) starts c rows (K-major) or c
+// elements (MN-major, c a multiple of 64: c / 64 column blocks) further on.
+template <int NP, int TNSP>
+__device__ __forceinline__ void wgmma_rows(float *acc, uint64_t da, uint64_t db, uint32_t b_block_bytes = 0)
 {
-    if (npad - n0 >= 32) {
-        tmem_ld32(taddr + (uint32_t)n0, raw);
-    } else {
-        uint32_t r16[16];
-        asm volatile("tcgen05.ld.sync.aligned.32x32b.x16.b32"
-                     "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-                     : "=r"(r16[0]), "=r"(r16[1]), "=r"(r16[2]), "=r"(r16[3]), "=r"(r16[4]), "=r"(r16[5]),
-                       "=r"(r16[6]), "=r"(r16[7]), "=r"(r16[8]), "=r"(r16[9]), "=r"(r16[10]), "=r"(r16[11]),
-                       "=r"(r16[12]), "=r"(r16[13]), "=r"(r16[14]), "=r"(r16[15])
-                     : "r"(taddr + (uint32_t)n0));
-        asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+    constexpr int C256 = NP & 256, C128 = NP & 128, C64 = NP & 64, C32 = NP & 32, C16 = NP & 16;
+    auto boff = [&](int c) -> uint64_t { return TNSP ? (uint64_t)((c / 64) * b_block_bytes >> 4) : (uint64_t)(c * 128 >> 4); };
+    if constexpr (C256 != 0) wgmma_n256<TNSP>(acc, da, db);
+    if constexpr (C128 != 0) wgmma_n128<TNSP>(acc + C256 / 2, da, db + boff(C256));
+    if constexpr (C64 != 0) wgmma_n64<TNSP>(acc + (C256 + C128) / 2, da, db + boff(C256 + C128));
+    if constexpr (C32 != 0) wgmma_n32<TNSP>(acc + (C256 + C128 + C64) / 2, da, db + boff(C256 + C128 + C64));
+    if constexpr (C16 != 0) wgmma_n16<TNSP>(acc + (C256 + C128 + C64 + C32) / 2, da, db + boff(C256 + C128 + C64 + C32));
+}
+
+// Epilogue staging: columns [64 p, 64 p + 64) of a warpgroup's accumulator -> its [64][TC_STG_LD] fp32 tile in shared memory
+// (row = accumulator row), so that each thread can then read one row's 32 consecutive columns.
+template <int NP>
+__device__ __forceinline__ void stage_acc(const float *acc, int p, float *stg)
+{
+    const int w = (threadIdx.x >> 5) & 3, l = threadIdx.x & 31;
+    const int r0 = 16 * w + (l >> 2), c0 = 2 * (l & 3);
 #pragma unroll
-        for (int j = 0; j < 16; ++j) { raw[j] = r16[j]; raw[16 + j] = 0u; }
+    for (int i = 0; i < NP / 2; i += 2) {
+        if (i / 32 != p) continue;
+        const int row = r0 + 8 * ((i >> 1) & 1), col = 8 * (i >> 2) + c0 - 64 * p;
+        *reinterpret_cast<float2 *>(stg + row * TC_STG_LD + col) = make_float2(acc[i], acc[i + 1]);
     }
 }
-// "stacked" accumulators (ConvTCArgs::stack): columns [0, npad) hold A_hi.B_hi + A_lo.B_hi, columns [npad, 2 npad) hold A_hi.B_lo
-__device__ __forceinline__ void tmem_ld_chunk_stacked(uint32_t taddr, int n0, int npad, uint32_t (&raw)[32])
+// 32 staged columns [32 h, 32 h + 32) of row r (16 valid ones when only 16 remain: zeros above)
+__device__ __forceinline__ void staged_row32(const float *stg, int r, int h, int nvalid, uint32_t (&raw)[32])
 {
-    uint32_t lo[32];
-    tmem_ld_chunk(taddr, n0, npad, raw);
-    tmem_ld_chunk(taddr + (uint32_t)npad, n0, npad, lo);
+    const float4 *sp = reinterpret_cast<const float4 *>(stg + r * TC_STG_LD + 32 * h);
 #pragma unroll
-    for (int j = 0; j < 32; ++j) raw[j] = __float_as_uint(__uint_as_float(raw[j]) + __uint_as_float(lo[j]));
-}
-
-// K-major, 128B-swizzled operand tile (rows of 128 bytes, 8-row groups 1024 bytes apart).
-// Bits: start>>4 [0,14) | LBO>>4 [16,30) | SBO>>4 [32,46) | version=1 [46,48) | layout=SWIZZLE_128B(2) [61,64)
-__device__ __forceinline__ uint64_t umma_smem_desc(uint32_t smem_addr)
-{
-    uint64_t d = 0;
-    d |= (uint64_t)((smem_addr & 0x3FFFFu) >> 4);
-    d |= (uint64_t)1 << 16;                 // LBO (ignored for swizzled K-major)
-    d |= (uint64_t)(1024 >> 4) << 32;       // SBO = 1024 B
-    d |= (uint64_t)1 << 46;                 // descriptor version (sm_100)
-    d |= (uint64_t)2 << 61;                 // SWIZZLE_128B
-    return d;
-}
-// The same descriptor in two words: lo = address field | LBO, hi = SBO | version | SWIZZLE_128B (a constant per operand kind).  Advancing
-// the operand by n bytes (n a multiple of 16, the result below 256 KB) is lo + n / 16.
-__device__ __forceinline__ uint32_t umma_desc_lo(uint32_t smem_addr) { return ((smem_addr & 0x3FFFFu) >> 4) | (1u << 16); }
-__device__ __forceinline__ uint64_t umma_desc(uint32_t lo, uint32_t hi) { return ((uint64_t)hi << 32) | lo; }
-constexpr uint32_t UMMA_HI_1024 = (1024u >> 4) | (1u << 14) | (2u << 29);      // upper word of umma_smem_desc(): SBO = 1024 B, version 1, SWIZZLE_128B
-// c=F32 [4,6)=1 | a=BF16 [7,10)=1 | b=BF16 [10,13)=1 | K-major A,B | N>>3 [17,23) | M>>4 [24,29)
-__device__ __forceinline__ uint32_t umma_idesc(int M, int N)
-{
-    return (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
+    for (int q = 0; q < 8; ++q) {
+        const float4 v = (q < 4 || nvalid >= 32) ? sp[q] : make_float4(0.f, 0.f, 0.f, 0.f);
+        raw[4 * q] = __float_as_uint(v.x); raw[4 * q + 1] = __float_as_uint(v.y);
+        raw[4 * q + 2] = __float_as_uint(v.z); raw[4 * q + 3] = __float_as_uint(v.w);
+    }
 }
 
 __device__ __forceinline__ float apply_act(float x, int act)
@@ -284,29 +318,6 @@ __device__ __forceinline__ void epilogue_std_math(const ConvTCArgs &a, float (&v
         for (int j = 0; j < 32; ++j) v[j] += r[j];
     }
 }
-// bias + standard epilogue math of one chunk, values only (the caller stores them): the out_tma path
-__device__ __forceinline__ void epilogue_values(const ConvTCArgs &a, const uint32_t (&raw)[32], int n0, int img, int y, int x, bool valid,
-                                                float (&v)[32])
-{
-    const float4 *bp = reinterpret_cast<const float4 *>(a.bias + n0);
-#pragma unroll
-    for (int q = 0; q < 8; ++q) {
-        const float4 b = bp[q];
-        v[4 * q + 0] = __uint_as_float(raw[4 * q + 0]) + b.x;
-        v[4 * q + 1] = __uint_as_float(raw[4 * q + 1]) + b.y;
-        v[4 * q + 2] = __uint_as_float(raw[4 * q + 2]) + b.z;
-        v[4 * q + 3] = __uint_as_float(raw[4 * q + 3]) + b.w;
-    }
-    epilogue_std_math(a, v, n0, img, y, x, valid);
-}
-__device__ __forceinline__ void tma_store_5d(const CUtensorMap *map, uint32_t src, int c0, int c1, int c2, int c3, int c4)
-{
-    // L2 evict_last: the tensor is the next layer's input and must stay in the 126 MB L2 like the lines of a plain st.global do
-    // (without the hint every consumer kernel got 3-5 us slower: its input came from HBM)
-    asm volatile("cp.async.bulk.tensor.5d.global.shared::cta.bulk_group.L2::cache_hint [%0, {%2, %3, %4, %5, %6}], [%1], %7;"
-                 ::"l"(map), "r"(src), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "r"(c4), "l"(0x14F0000000000000ull) : "memory");
-}
-
 __device__ __forceinline__ void epilogue_chunk(const ConvTCArgs &a, const uint32_t (&raw)[32], int n0, size_t pix, int img,
                                                int y, int x)
 {

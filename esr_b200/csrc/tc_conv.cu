@@ -1,506 +1,208 @@
-// tc_conv.cu -- 3x3 / 1x1 convolution as an implicit GEMM on the 5th-gen tensor cores (sm_100a).
+// tc_conv.cu -- 3x3 / 1x1 convolution as an implicit GEMM on the Hopper tensor cores (sm_90a, wgmma).
 //
 //   D[128 pixels, Cout] += A[128 pixels, 64 ch of one tap] * B[Cout, 64]^T      per K-block (tap x 64-channel chunk)
 //
 // * Activations live in HBM as "split bf16" NHWC tensors (value = hi + lo).  A K-block's A tile is ONE TMA box
 //   (64 ch, TW, TH, 1 image, 1 plane) taken at the tap's (dy, dx) shift; out-of-image coordinates are zero-filled
 //   by TMA, which is exactly the conv's zero padding.  The box lands in shared memory in the 128B-swizzled K-major
-//   layout that tcgen05.mma consumes, so no thread touches the operands.
+//   layout that wgmma reads, so no thread touches the operands.
 // * Channel concatenation (torch.cat in the reference) is a K-split over up to 3 source tensors.
-// * fp32 parity: three bf16 MMAs per K-step (lo*hi + hi*lo + hi*hi) accumulate in fp32 in TMEM => ~2^-17 relative
+// * fp32 parity: three bf16 MMAs per K-step (lo*hi + hi*lo + hi*hi) accumulate in fp32 registers => ~2^-17 relative
 //   operand error instead of bf16's 2^-9 (the reference network is fp32-only).
-// * Warp roles: warp 0 = TMA producer, warp 1 = TMEM owner + single-thread MMA issuer, warps 2..5 = epilogue
-//   (tcgen05.ld -> bias / residual / activation / GRU gating -> split-bf16 or fp32 NHWC stores).
-// * mbarrier ring: full[s] (TMA -> MMA), empty[s] (tcgen05.commit -> TMA), accum_full (tcgen05.commit -> epilogue).
+// * Warp roles: warps 0-7 = two consumer warpgroups (pixel rows 0-63 / 64-127 of the tile, accumulators in registers,
+//   then the epilogue: staging through shared memory -> bias / residual / activation / GRU gating -> split-bf16 or fp32
+//   stores); warp 8 = TMA producer.
+// * mbarrier ring: full[s] (TMA -> consumers), empty[s] (one arrival per consumer warp once its MMAs on s retired -> TMA).
 //
 // Reference layers served: every Conv2d of models/model.py at feature resolution (Cin multiple of 64), the ConvGRU
 // gates (models/submodules.py:496-514) and the DCNv2 contraction (models/DCNv2/src/cuda/dcn_v2_cuda.cu:90-92).
 #include "tc_common.cuh"
+#include <algorithm>
 #include <cstdlib>
 
 namespace esr {
 
+constexpr int TC_THREADS = 288;
 
 // ------------------------------------------------------------------------------------------------
-// the kernel: one CTA = one tile of 128 output pixels (TH x TW) of one image, all output channels
+// Persistent conv body: the CTA walks tiles tile0, tile0 + step, ... of one layer (128 output pixels (TH x TW) of one image x
+// all NP (= npad) output channels each).  The TMA producer streams K-blocks across tile boundaries through the ring, so the
+// loads of tile i+1 overlap the epilogue of tile i; the ring position (s, ph) of each role persists across tiles and calls.
+// The epilogue stages accumulators in a dedicated area beside the ring (the ring is already refilling).
 // ------------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(TC_THREADS, 2) k_conv_tc(const __grid_constant__ ConvTCArgs a)
+struct TcSmem {
+    uint32_t ring, stage_stride, bar_full, bar_empty;   // shared-memory addresses
+    float *stg;                                         // epilogue staging: [2 warpgroups][64][TC_STG_LD] fp32
+    int stages;
+};
+struct TcRing { uint32_t s = 0, ph = 0; };
+
+static size_t tc_smem_bytes(int npad, int stages)
 {
-    PDL_LAUNCH_DEPENDENTS();
+    return 1024 + (size_t)stages * (2 * TC_A_BYTES + 2 * (size_t)npad * 128) + 2 * TC_STG_BYTES + 16 * (size_t)stages + 64;
+}
+__device__ __forceinline__ TcSmem tc_smem_layout(int np_max, int stages)
+{
     extern __shared__ uint8_t smem_raw[];
-    const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;     // SWIZZLE_128B needs 1024-B alignment
-    const uint32_t b_bytes = (uint32_t)a.npad * 128u;
-    const uint32_t stage_bytes = 2u * TC_A_BYTES + 2u * b_bytes;
-    const uint32_t bar_base = smem_base + (uint32_t)a.stages * stage_bytes;
-    // barriers: full[stages], empty[stages], accum_full, then the TMEM base address slot
-    const uint32_t bar_full = bar_base, bar_empty = bar_base + 8u * a.stages, bar_accum = bar_base + 16u * a.stages;
-    const uint32_t tmem_slot = bar_accum + 8u;
-
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    uint32_t tmem_cols = 32;
-    while ((int)tmem_cols < (a.stack ? 2 * a.npad : a.npad)) tmem_cols <<= 1;
-
-    // tile -> (image, y0, x0)
-    const int tiles_per_img = a.tiles_x * a.tiles_y;
-    const int img = blockIdx.x / tiles_per_img;
-    const int trem = blockIdx.x - img * tiles_per_img;
-    const int y0 = (trem / a.tiles_x) * a.TH, x0 = (trem % a.tiles_x) * a.TW;
-
+    TcSmem m;
+    m.ring = (smem_u32(smem_raw) + 1023u) & ~1023u;                    // SWIZZLE_128B needs 1024-B alignment
+    m.stage_stride = 2u * TC_A_BYTES + 2u * (uint32_t)np_max * 128u;
+    const uint32_t stg = m.ring + (uint32_t)stages * m.stage_stride;
+    m.stg = reinterpret_cast<float *>(smem_raw + (stg - smem_u32(smem_raw)));
+    m.bar_full = stg + 2u * TC_STG_BYTES;
+    m.bar_empty = m.bar_full + 8u * stages;
+    m.stages = stages;
+    return m;
+}
+__device__ __forceinline__ void tc_init_barriers(const TcSmem &m)
+{
     if (threadIdx.x == 0) {
-        for (int s = 0; s < a.stages; ++s) { mbar_init(bar_full + 8u * s, 1); mbar_init(bar_empty + 8u * s, 1); }
-        mbar_init(bar_accum, 1);
+        for (int s = 0; s < m.stages; ++s) { mbar_init(m.bar_full + 8u * s, 1); mbar_init(m.bar_empty + 8u * s, 8); }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
-    if (warp == 1) tmem_alloc(tmem_slot, tmem_cols);
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    uint32_t tmem_base;
-    asm volatile("ld.shared.b32 %0, [%1];" : "=r"(tmem_base) : "r"(tmem_slot));
-    PDL_WAIT();                      // everything above is CTA-local set-up; global memory only from here on
+}
 
-    if (warp == 0) {
-        // ===================== TMA producer =====================
+template <int NP>
+__device__ __forceinline__ void conv_tiles(const ConvTCArgs &a, int tile0, int step, const TcSmem &m, TcRing &ring)
+{
+    constexpr uint32_t b_bytes = (uint32_t)NP * 128u;
+    constexpr uint32_t tx_bytes = 2u * TC_A_BYTES + 2u * b_bytes;
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int tiles_per_img = a.tiles_x * a.tiles_y, n_tiles = a.n_img * tiles_per_img;
+
+    if (warp == 8) {
+        // ===================== TMA producer (one elected lane; the others idle until the caller's next barrier) =====================
         if (elect_one_sync()) {
-            uint32_t s = 0, ph = 0;
-            int src = 0, chunk_base = 0;
-            for (int kb = 0; kb < a.nkb; ++kb) {
-                const int gchunk = kb / a.ntaps, tap = kb - gchunk * a.ntaps;
-                while (gchunk >= a.chunk_end[src]) { chunk_base = a.chunk_end[src]; ++src; }
-                const int dy = a.ntaps == 9 ? tap / 3 - 1 : 0, dx = a.ntaps == 9 ? tap % 3 - 1 : 0;
-                const int simg = a.src_img[src] ? a.src_img[src][img] : img;
-                mbar_wait(bar_empty + 8u * s, ph ^ 1u);
-                mbar_expect_tx(bar_full + 8u * s, stage_bytes);
-                const uint32_t st = smem_base + s * stage_bytes;
-                const int c0 = (gchunk - chunk_base) * 64;
-                tma_load_5d(&a.amap[src], bar_full + 8u * s, st, c0, x0 + dx, y0 + dy, simg, 0);
-                tma_load_5d(&a.amap[src], bar_full + 8u * s, st + TC_A_BYTES, c0, x0 + dx, y0 + dy, simg, 1);
-                tma_load_3d(&a.bmap, bar_full + 8u * s, st + 2u * TC_A_BYTES, 0, 0, kb);
-                tma_load_3d(&a.bmap, bar_full + 8u * s, st + 2u * TC_A_BYTES + b_bytes, 0, 0, a.nkb + kb);
-                if (++s == (uint32_t)a.stages) { s = 0; ph ^= 1u; }
-            }
-        }
-    } else if (warp == 1) {
-        // ===================== MMA issuer (one thread) =====================
-        if (elect_one_sync()) {
-            const uint32_t idesc = umma_idesc(TC_BLOCK_M, a.npad), idesc2 = umma_idesc(TC_BLOCK_M, 2 * a.npad);
-            uint32_t s = 0, ph = 0;
-            for (int kb = 0; kb < a.nkb; ++kb) {
-                mbar_wait(bar_full + 8u * s, ph);
-                tc_fence_after();
-                const uint32_t st = smem_base + s * stage_bytes;
-                const uint32_t a_hi = st, a_lo = st + TC_A_BYTES, b_hi = st + 2u * TC_A_BYTES, b_lo = b_hi + b_bytes;
-                if (a.stack) {
-                    // B_hi and B_lo are adjacent in the stage: ONE descriptor over 2 npad rows = [B_hi; B_lo]
-#pragma unroll
-                    for (int k = 0; k < 4; ++k) {
-                        const uint64_t dah = umma_desc(umma_desc_lo(a_hi) + 2u * k, UMMA_HI_1024), dal = umma_desc(umma_desc_lo(a_lo) + 2u * k, UMMA_HI_1024);
-                        const uint64_t dbh = umma_desc(umma_desc_lo(b_hi) + 2u * k, UMMA_HI_1024);
-                        umma_bf16(tmem_base, dah, dbh, idesc2, (kb | k) != 0 ? 1u : 0u);   // cols [0,npad) += A_hi B_hi, [npad,2npad) += A_hi B_lo
-                        umma_bf16(tmem_base, dal, dbh, idesc, 1u);                          // cols [0,npad) += A_lo B_hi
-                    }
-                } else {
-#pragma unroll
-                    for (int k = 0; k < 4; ++k) {                       // 4 x (K = 16 bf16 = 32 bytes) per 128-byte row
-                        const uint64_t dah = umma_desc(umma_desc_lo(a_hi) + 2u * k, UMMA_HI_1024), dal = umma_desc(umma_desc_lo(a_lo) + 2u * k, UMMA_HI_1024);
-                        const uint64_t dbh = umma_desc(umma_desc_lo(b_hi) + 2u * k, UMMA_HI_1024), dbl = umma_desc(umma_desc_lo(b_lo) + 2u * k, UMMA_HI_1024);
-                        umma_bf16(tmem_base, dal, dbh, idesc, (kb | k) != 0 ? 1u : 0u);   // small terms first
-                        umma_bf16(tmem_base, dah, dbl, idesc, 1u);
-                        umma_bf16(tmem_base, dah, dbh, idesc, 1u);
-                    }
+            uint32_t s = ring.s, ph = ring.ph;
+            for (int tile = tile0; tile < n_tiles; tile += step) {
+                const int img = tile / tiles_per_img, trem = tile - img * tiles_per_img;
+                const int y0 = (trem / a.tiles_x) * a.TH, x0 = (trem % a.tiles_x) * a.TW;
+                int src = 0, chunk_base = 0;
+                for (int kb = 0; kb < a.nkb; ++kb) {
+                    const int gchunk = kb / a.ntaps, tap = kb - gchunk * a.ntaps;
+                    while (gchunk >= a.chunk_end[src]) { chunk_base = a.chunk_end[src]; ++src; }
+                    const int dy = a.ntaps == 9 ? tap / 3 - 1 : 0, dx = a.ntaps == 9 ? tap % 3 - 1 : 0;
+                    const int simg = a.src_img[src] ? a.src_img[src][img] : img;
+                    mbar_wait(m.bar_empty + 8u * s, ph ^ 1u);
+                    mbar_expect_tx(m.bar_full + 8u * s, tx_bytes);
+                    const uint32_t st = m.ring + s * m.stage_stride;
+                    const int c0 = (gchunk - chunk_base) * 64;
+                    tma_load_5d(&a.amap[src], m.bar_full + 8u * s, st, c0, x0 + dx, y0 + dy, simg, 0);
+                    tma_load_5d(&a.amap[src], m.bar_full + 8u * s, st + TC_A_BYTES, c0, x0 + dx, y0 + dy, simg, 1);
+                    tma_load_3d(&a.bmap, m.bar_full + 8u * s, st + 2u * TC_A_BYTES, 0, 0, kb);
+                    tma_load_3d(&a.bmap, m.bar_full + 8u * s, st + 2u * TC_A_BYTES + b_bytes, 0, 0, a.nkb + kb);
+                    if (++s == (uint32_t)m.stages) { s = 0; ph ^= 1u; }
                 }
-                umma_commit(bar_empty + 8u * s);                    // frees the stage once these MMAs retire
-                if (++s == (uint32_t)a.stages) { s = 0; ph ^= 1u; }
             }
-            umma_commit(bar_accum);                                 // accumulator complete
+            ring.s = s; ring.ph = ph;
         }
-    } else {
-        // ===================== epilogue (4 warps, one TMEM lane quadrant each) =====================
-        const int quad = warp & 3;                                  // tcgen05.ld: warp w may touch lanes 32*(w%4)..+31
-        const int m = quad * 32 + lane;                             // accumulator row = pixel within the tile
-        const int y = y0 + m / a.TW, x = x0 + m % a.TW;
+        return;
+    }
+
+    // ===================== consumers: warpgroup wg owns tile rows [64 wg, 64 wg + 64) =====================
+    const int wg = warp >> 2;
+    float *stg = m.stg + wg * (TC_STG_BYTES / 4);
+    const int r = threadIdx.x & 63, h = (threadIdx.x >> 6) & 1;
+    uint32_t s = ring.s, ph = ring.ph;
+    for (int tile = tile0; tile < n_tiles; tile += step) {
+        const int img = tile / tiles_per_img, trem = tile - img * tiles_per_img;
+        const int y0 = (trem / a.tiles_x) * a.TH, x0 = (trem % a.tiles_x) * a.TW;
+        float acc[NP / 2];
+#pragma unroll
+        for (int i = 0; i < NP / 2; ++i) acc[i] = 0.0f;
+        uint32_t prev = 0;
+        for (int kb = 0; kb < a.nkb; ++kb) {
+            mbar_wait(m.bar_full + 8u * s, ph);
+            const uint32_t st = m.ring + s * m.stage_stride;
+            const uint64_t dah = wgmma_desc(st + (uint32_t)wg * 8192u), dal = wgmma_desc(st + TC_A_BYTES + (uint32_t)wg * 8192u);
+            const uint64_t dbh = wgmma_desc(st + 2u * TC_A_BYTES), dbl = wgmma_desc(st + 2u * TC_A_BYTES + b_bytes);
+            acc_fence<NP / 2>(acc);
+            wgmma_fence();
+#pragma unroll
+            for (int k = 0; k < 4; ++k) {                           // 4 x (K = 16 bf16 = 32 bytes) per 128-byte row
+                wgmma_rows<NP, 0>(acc, dal + 2 * k, dbh + 2 * k);   // small terms first
+                wgmma_rows<NP, 0>(acc, dah + 2 * k, dbl + 2 * k);
+                wgmma_rows<NP, 0>(acc, dah + 2 * k, dbh + 2 * k);
+            }
+            wgmma_commit();
+            wgmma_wait<1>();                                        // the previous K-block's MMAs have retired: free its stage
+            acc_fence<NP / 2>(acc);
+            if (kb > 0 && lane == 0) mbar_arrive(m.bar_empty + 8u * prev);
+            prev = s;
+            if (++s == (uint32_t)m.stages) { s = 0; ph ^= 1u; }
+        }
+        wgmma_wait<0>();
+        acc_fence<NP / 2>(acc);
+        if (lane == 0) mbar_arrive(m.bar_empty + 8u * prev);      // the tile's last stage
+
+        // ===================== epilogue: thread = (tile row r, 32-column half h) per 64-column pass =====================
+        const int mrow = wg * 64 + r;                               // accumulator row = pixel within the tile
+        const int y = y0 + mrow / a.TW, x = x0 + mrow % a.TW;
         const bool valid = (y < a.H) && (x < a.W);
         const size_t pix = ((size_t)img * a.H + (valid ? y : 0)) * a.W + (valid ? x : 0);
-        mbar_wait_backoff(bar_accum, 0);   // four warps idle for the whole main loop: poll with back-off
-        tc_fence_after();
-        const uint32_t taddr = tmem_base + ((uint32_t)(quad * 32) << 16);
-        for (int n0 = 0; n0 < a.npad; n0 += 32) {
-            uint32_t raw[32];
-            if (a.stack) tmem_ld_chunk_stacked(taddr, n0, a.npad, raw);
-            else tmem_ld_chunk(taddr, n0, a.npad, raw);
-            if (valid) epilogue_chunk(a, raw, n0, pix, img, y, x);
-            __syncwarp();
+#pragma unroll
+        for (int p = 0; p < (NP + 63) / 64; ++p) {
+            stage_acc<NP>(acc, p, stg);
+            named_sync(2 + wg, 128);
+            const int n0 = 64 * p + 32 * h;
+            if (n0 < NP) {
+                uint32_t raw[32];
+                staged_row32(stg, r, h, NP - n0, raw);
+                if (valid) epilogue_chunk(a, raw, n0, pix, img, y, x);
+            }
+            named_sync(2 + wg, 128);
         }
     }
-
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 1) { tc_fence_after(); tmem_dealloc(tmem_base, tmem_cols); }
+    ring.s = s; ring.ph = ph;
 }
 
-// ------------------------------------------------------------------------------------------------
-// Persistent variant for the wide layers (N > 128: one stage ring fills most of the shared memory, so only ONE CTA fits per
-// SM and k_conv_tc's epilogue -- 6-7 chunks of tcgen05.ld + bias/residual/activation + stores -- runs with the tensor core
-// idle).  Here a CTA walks tiles blockIdx.x, blockIdx.x + gridDim.x, ... with TWO accumulators in TMEM (2 x 256 columns):
-// the MMA thread starts tile i+1 in the other accumulator while the epilogue warps drain tile i; the TMA producer simply
-// streams K-blocks across tile boundaries.  Same operand order, same epilogue code: results are bit-identical to k_conv_tc.
-// ------------------------------------------------------------------------------------------------
-constexpr uint32_t TCP_STG_PLANE = 32 * 64, TCP_STG_BUF = 2 * TCP_STG_PLANE;   // per-warp staging of the TMA-store epilogue (split outputs)
-__global__ void __launch_bounds__(TC_THREADS, 1) k_conv_tc_persist(const __grid_constant__ ConvTCArgs a)
+// one layer: grid = min(tiles, resident CTAs); CTA b takes tiles b, b + gridDim.x, ...
+template <int NP>
+__global__ void __launch_bounds__(TC_THREADS, NP <= 64 ? 2 : 1) k_conv_tc(const __grid_constant__ ConvTCArgs a)
 {
     PDL_LAUNCH_DEPENDENTS();
-    extern __shared__ uint8_t smem_raw[];
-    const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
-    const uint32_t b_bytes = (uint32_t)a.npad * 128u;
-    const uint32_t stage_bytes = 2u * TC_A_BYTES + 2u * b_bytes;
-    const uint32_t stg_ring = smem_base + (uint32_t)a.stages * stage_bytes;      // out_tma: [4 warps][2 buffers][2 planes][32 px x 64 B] (tc_conv_halo.cu)
-    const uint32_t bar_base = stg_ring + (a.out_tma ? 4u * 2u * TCP_STG_BUF : 0u);
-    const uint32_t bar_full = bar_base, bar_empty = bar_base + 8u * a.stages;
-    const uint32_t bar_afull = bar_base + 16u * a.stages, bar_aempty = bar_afull + 16u;      // per accumulator
-    const uint32_t tmem_slot = bar_aempty + 16u;
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int tiles_per_img = a.tiles_x * a.tiles_y, n_tiles = a.n_img * tiles_per_img;
-
-    if (threadIdx.x == 0) {
-        for (int s = 0; s < a.stages; ++s) { mbar_init(bar_full + 8u * s, 1); mbar_init(bar_empty + 8u * s, 1); }
-        for (int i = 0; i < 2; ++i) { mbar_init(bar_afull + 8u * i, 1); mbar_init(bar_aempty + 8u * i, 128); }
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    if (warp == 1) tmem_alloc(tmem_slot, 512);
-    tc_fence_before();
-    __syncthreads();
-    tc_fence_after();
-    uint32_t tmem_base;
-    asm volatile("ld.shared.b32 %0, [%1];" : "=r"(tmem_base) : "r"(tmem_slot));
+    const TcSmem m = tc_smem_layout(NP, a.stages);
+    tc_init_barriers(m);
     PDL_WAIT();                      // everything above is CTA-local set-up; global memory only from here on
+    TcRing ring;
+    conv_tiles<NP>(a, blockIdx.x, gridDim.x, m, ring);
+}
 
-    if (warp == 0) {
-        if (elect_one_sync()) {
-            uint32_t s = 0, ph = 0;
-            long long *tr = (a.trace && blockIdx.x == 0) ? a.trace : nullptr;
-            int tn = 0;
-            for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
-                const int img = tile / tiles_per_img, trem = tile - img * tiles_per_img;
-                const int y0 = (trem / a.tiles_x) * a.TH, x0 = (trem % a.tiles_x) * a.TW;
-                int src = 0, chunk_base = 0;
-                for (int kb = 0; kb < a.nkb; ++kb) {
-                    const int gchunk = kb / a.ntaps, tap = kb - gchunk * a.ntaps;
-                    while (gchunk >= a.chunk_end[src]) { chunk_base = a.chunk_end[src]; ++src; }
-                    const int dy = a.ntaps == 9 ? tap / 3 - 1 : 0, dx = a.ntaps == 9 ? tap % 3 - 1 : 0;
-                    const int simg = a.src_img[src] ? a.src_img[src][img] : img;
-                    mbar_wait(bar_empty + 8u * s, ph ^ 1u);
-                    if (tr && tn < TRACE_N) tr[tn * 8 + 0] = clock64();
-                    mbar_expect_tx(bar_full + 8u * s, stage_bytes - ((a.diag & 1) ? b_bytes : 0u) - ((a.diag & 2) ? (uint32_t)TC_A_BYTES : 0u));
-                    const uint32_t st = smem_base + s * stage_bytes;
-                    const int c0 = (gchunk - chunk_base) * 64;
-                    tma_load_5d(&a.amap[src], bar_full + 8u * s, st, c0, x0 + dx, y0 + dy, simg, 0);
-                    if (!(a.diag & 2)) tma_load_5d(&a.amap[src], bar_full + 8u * s, st + TC_A_BYTES, c0, x0 + dx, y0 + dy, simg, 1);
-                    tma_load_3d(&a.bmap, bar_full + 8u * s, st + 2u * TC_A_BYTES, 0, 0, kb);
-                    if (!(a.diag & 1)) tma_load_3d(&a.bmap, bar_full + 8u * s, st + 2u * TC_A_BYTES + b_bytes, 0, 0, a.nkb + kb);
-                    if (tr && tn < TRACE_N) { tr[tn * 8 + 1] = clock64(); ++tn; }
-                    if (++s == (uint32_t)a.stages) { s = 0; ph ^= 1u; }
-                }
-            }
-        }
-    } else if (warp == 1) {
-        if (elect_one_sync()) {
-            const uint32_t idesc = umma_idesc(TC_BLOCK_M, a.npad), idesc2 = umma_idesc(TC_BLOCK_M, 2 * a.npad);
-            uint32_t s = 0, ph = 0;
-            int it = 0;
-            long long *tr = (a.trace && blockIdx.x == 0) ? a.trace : nullptr;
-            int tn = 0;
-            for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x, ++it) {
-                const uint32_t ai = (uint32_t)(it & 1), aph = (uint32_t)((it >> 1) & 1);
-                mbar_wait(bar_aempty + 8u * ai, aph ^ 1u);          // the epilogue of tile it-2 has drained this accumulator
-                tc_fence_after();
-                const uint32_t acc = tmem_base + ai * 256u;
-                for (int kb = 0; kb < a.nkb; ++kb) {
-                    if (tr && tn < TRACE_N) tr[tn * 8 + 2] = clock64();
-                    mbar_wait(bar_full + 8u * s, ph);
-                    tc_fence_after();
-                    if (tr && tn < TRACE_N) tr[tn * 8 + 3] = clock64();
-                    const uint32_t st = smem_base + s * stage_bytes;
-                    const uint32_t a_hi = st, a_lo = st + TC_A_BYTES, b_hi = st + 2u * TC_A_BYTES, b_lo = b_hi + b_bytes;
-#pragma unroll
-                    for (int k = 0; k < 4; ++k) {
-                        const uint64_t dah = umma_desc(umma_desc_lo(a_hi) + 2u * k, UMMA_HI_1024), dal = umma_desc(umma_desc_lo(a_lo) + 2u * k, UMMA_HI_1024);
-                        const uint64_t dbh = umma_desc(umma_desc_lo(b_hi) + 2u * k, UMMA_HI_1024), dbl = umma_desc(umma_desc_lo(b_lo) + 2u * k, UMMA_HI_1024);
-                        if (a.stack) {
-                            umma_bf16(acc, dah, dbh, idesc2, (kb | k) != 0 ? 1u : 0u);   // [B_hi; B_lo] as one 2 npad-row operand
-                            umma_bf16(acc, dal, dbh, idesc, 1u);
-                        } else if (!(a.diag & 4)) {
-                            umma_bf16(acc, dal, dbh, idesc, (kb | k) != 0 ? 1u : 0u);
-                            umma_bf16(acc, dah, dbl, idesc, 1u);
-                            umma_bf16(acc, dah, dbh, idesc, 1u);
-                        } else {
-                            umma_bf16(acc, dah, dbh, idesc, (kb | k) != 0 ? 1u : 0u);   // measurement aid: one pass only
-                        }
-                    }
-                    umma_commit(bar_empty + 8u * s);
-                    if (tr && tn < TRACE_N) { tr[tn * 8 + 4] = clock64(); ++tn; }
-                    if (++s == (uint32_t)a.stages) { s = 0; ph ^= 1u; }
-                }
-                umma_commit(bar_afull + 8u * ai);
-            }
-        }
-    } else {
-        const int quad = warp & 3;
-        const int m = quad * 32 + lane;
-        int it = 0;
-        uint32_t stg_n = 0;
-        for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x, ++it) {
-            const uint32_t ai = (uint32_t)(it & 1), aph = (uint32_t)((it >> 1) & 1);
-            const int img = tile / tiles_per_img, trem = tile - img * tiles_per_img;
-            const int y0 = (trem / a.tiles_x) * a.TH, x0 = (trem % a.tiles_x) * a.TW;
-            const int y = y0 + m / a.TW, x = x0 + m % a.TW;
-            const bool valid = (y < a.H) && (x < a.W);
-            const size_t pix = ((size_t)img * a.H + (valid ? y : 0)) * a.W + (valid ? x : 0);
-            mbar_wait_backoff(bar_afull + 8u * ai, aph);
-            tc_fence_after();
-            if (a.trace && blockIdx.x == 0 && threadIdx.x == 64 && it < TRACE_N) a.trace[it * 8 + 5] = clock64();
-            const uint32_t taddr = tmem_base + ai * 256u + ((uint32_t)(quad * 32) << 16);
-            for (int n0 = 0; n0 < a.npad; n0 += 32) {
-                uint32_t raw[32];
-                if (a.diag & 16) continue;                          // measurement aid: no TMEM reads, no stores
-                if (a.stack) tmem_ld_chunk_stacked(taddr, n0, a.npad, raw);
-                else tmem_ld_chunk(taddr, n0, a.npad, raw);
-                if (a.out_tma == 1 && !(a.diag & 8)) {
-                    // staged epilogue as in k_conv_tc_halo: this warp's 32 pixels x 32 channels -> swizzled shared memory -> TMA store
-                    const uint32_t buf = stg_ring + ((uint32_t)quad * 2u + (stg_n & 1u)) * TCP_STG_BUF;
-                    if (lane == 0) asm volatile("cp.async.bulk.wait_group.read 1;" ::: "memory");
-                    __syncwarp();
-                    float v[32];
-                    epilogue_values(a, raw, n0, img, y, x, valid, v);
-                    uint32_t hw[16], lw[16];
-#pragma unroll
-                    for (int e = 0; e < 16; ++e) split_pack2(v[2 * e], v[2 * e + 1], hw[e], lw[e]);
-                    const uint32_t row = buf + (uint32_t)lane * 64u, sw = ((uint32_t)lane >> 1) & 3u;
-#pragma unroll
-                    for (int q = 0; q < 4; ++q) {
-                        const uint32_t o = row + (((uint32_t)q ^ sw) << 4);
-                        asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(o), "r"(hw[4 * q]), "r"(hw[4 * q + 1]), "r"(hw[4 * q + 2]), "r"(hw[4 * q + 3]) : "memory");
-                        asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(o + TCP_STG_PLANE), "r"(lw[4 * q]), "r"(lw[4 * q + 1]), "r"(lw[4 * q + 2]), "r"(lw[4 * q + 3]) : "memory");
-                    }
-                    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-                    __syncwarp();
-                    if (lane == 0) {
-                        const int rows = 32 / a.TW, yq = y0 + quad * rows;
-                        tma_store_5d(&a.omap, buf, a.out_coff + n0, x0, yq, img, 0);
-                        tma_store_5d(&a.omap, buf + TCP_STG_PLANE, a.out_coff + n0, x0, yq, img, 1);
-                        asm volatile("cp.async.bulk.commit_group;" ::: "memory");
-                    }
-                    ++stg_n;
-                } else
-                if (valid && !(a.diag & 8)) epilogue_chunk(a, raw, n0, pix, img, y, x);
-                else if (a.diag & 8) { if (raw[0] == 0x7fc12345u && raw[31] == 0x7fc54321u) a.out_f32[0] = 1.0f; }   // keep the loads alive
-                __syncwarp();
-            }
-            tc_fence_before();                                       // this thread's TMEM reads are done: release the accumulator
-            if (a.trace && blockIdx.x == 0 && threadIdx.x == 64 && it < TRACE_N) a.trace[it * 8 + 6] = clock64();
-            asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar_aempty + 8u * ai) : "memory");
-        }
-        if (a.out_tma == 1 && lane == 0) asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
-    }
-
-    tc_fence_before();
+// ------------------------------------------------------------------------------------------------
+// The whole ConvGRU recurrence of a sequence batch in ONE cooperative launch: phases 2g (update|reset gates, N = 128, epilogue
+// z -> z_buf, h*r -> rh) and 2g + 1 (candidate, N = 64, epilogue h' = h (1 - z) + tanh(.) z) of step g, each a persistent pass
+// over the step's tiles, separated by a grid barrier.  The next phase's TMA loads read what other CTAs stored with ordinary
+// stores, so every thread fences its stores into the async proxy before the barrier and after it.
+// ------------------------------------------------------------------------------------------------
+__device__ __forceinline__ void grid_barrier(unsigned int *ctr, unsigned int target)
+{
+    asm volatile("fence.proxy.async.global;" ::: "memory");
     __syncthreads();
-    if (warp == 1) { tc_fence_after(); tmem_dealloc(tmem_base, 512); }
-}
-
-// ------------------------------------------------------------------------------------------------
-// CTA-pair variant of the persistent kernel: clusters of two CTAs (the two SMs of a TPC) run ONE tcgen05.mma.cta_group::2 over
-// two adjacent pixel tiles (M = 2 x 128).  Each CTA stages only its own A tile and HALF of the weight tile (rows
-// [rank * npad/2, +npad/2)); the tensor cores of both SMs read both halves.  Per CTA a stage shrinks from 32 KB + 2 npad 128 B
-// to 32 KB + npad 128 B, which is what buys pipeline depth: measured on B200 (profiles/r2_notes.md) the single-CTA kernel is
-// bound by the TMA round trip (~2200 cycles) divided by the stages in flight -- 2 stages at N = 192, 4 at N = 64 -- not by
-// bytes or MMA issue.  Here N = 192 runs 4 stages deep, N = 64 five.
-// Protocol (S stages, two accumulators in TMEM as in k_conv_tc_persist):
-//   * every CTA: TMA producer -> own full[s]; own empty[s] is signalled by the leader's tcgen05.commit (multicast to both CTAs);
-//   * rank 1: one thread forwards "my stage s has landed" to the leader's pfull[s] (remote mbarrier arrive);
-//   * rank 0 (leader): one thread issues the MMAs once full[s] and pfull[s] are complete; commits multicast to both CTAs'
-//     empty[s] / afull[acc];
-//   * epilogue warps of both CTAs drain their own 128 TMEM lanes and arrive (one lane per warp) on the LEADER's aempty[acc].
-// Same operand order per output element as k_conv_tc / k_conv_tc_persist => bit-identical results.
-// ------------------------------------------------------------------------------------------------
-__device__ __forceinline__ void tmem_alloc_pair(uint32_t dst_smem, uint32_t cols)
-{
-    asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(dst_smem), "r"(cols) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc_pair(uint32_t addr, uint32_t cols)
-{
-    asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(addr), "r"(cols) : "memory");
-}
-__device__ __forceinline__ void umma_bf16_pair(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accum)
-{
-    asm volatile(
-        "{\n\t"
-        ".reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t"
-        "}" ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accum) : "memory");
-}
-__device__ __forceinline__ void umma_commit_pair(uint32_t bar)
-{
-    asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;"
-                 ::"r"(bar), "h"((uint16_t)3) : "memory");
-}
-
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(TC_THREADS, 1) k_conv_tc_pair(const __grid_constant__ ConvTCArgs a)
-{
-    extern __shared__ uint8_t smem_raw[];
-    const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
-    const uint32_t bh_bytes = (uint32_t)a.npad * 64u;                 // one plane of this CTA's HALF weight tile (npad/2 rows)
-    const uint32_t stage_bytes = 2u * TC_A_BYTES + 2u * bh_bytes;
-    const uint32_t bar_base = smem_base + (uint32_t)a.stages * stage_bytes;
-    const uint32_t bar_full = bar_base, bar_empty = bar_base + 8u * a.stages, bar_pfull = bar_base + 16u * a.stages;
-    const uint32_t bar_afull = bar_base + 24u * a.stages, bar_aempty = bar_afull + 16u;
-    const uint32_t tmem_slot = bar_aempty + 16u;
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const uint32_t rank = pair_rank();
-    const int tiles_per_img = a.tiles_x * a.tiles_y, n_tiles = a.n_img * tiles_per_img;
-    const int n_pairs = (n_tiles + 1) >> 1, pair0 = (int)(blockIdx.x >> 1), pair_step = (int)(gridDim.x >> 1);
-
     if (threadIdx.x == 0) {
-        for (int s = 0; s < a.stages; ++s) {
-            mbar_init(bar_full + 8u * s, 1); mbar_init(bar_empty + 8u * s, 1); mbar_init(bar_pfull + 8u * s, 1);
-        }
-        for (int i = 0; i < 2; ++i) { mbar_init(bar_afull + 8u * i, 1); mbar_init(bar_aempty + 8u * i, 8); }   // 4 + 4 epilogue warps
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+        __threadfence();
+        atomicAdd(ctr, 1u);
+        unsigned int v;
+        do {
+            asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(ctr) : "memory");
+            if (v < target) __nanosleep(32);
+        } while (v < target);
     }
-    if (warp == 1) tmem_alloc_pair(tmem_slot, 512);
-    tc_fence_before();
-    pair_sync();
-    tc_fence_after();
-    uint32_t tmem_base;
-    asm volatile("ld.shared.b32 %0, [%1];" : "=r"(tmem_base) : "r"(tmem_slot));
+    __syncthreads();
+    asm volatile("fence.proxy.async.global;" ::: "memory");
+}
 
-    if (warp == 0) {
-        // ===================== TMA producer (both CTAs): own A tile + own half of the weights =====================
-        if (elect_one_sync()) {
-            uint32_t s = 0, ph = 0;
-            const int brow = (int)rank * (a.npad >> 1);
-            long long *tr = (a.trace && blockIdx.x == 0) ? a.trace : nullptr;
-            int tn = 0;
-            for (int pr = pair0; pr < n_pairs; pr += pair_step) {
-                const int tile = min(2 * pr + (int)rank, n_tiles - 1);
-                const int img = tile / tiles_per_img, trem = tile - img * tiles_per_img;
-                const int y0 = (trem / a.tiles_x) * a.TH, x0 = (trem % a.tiles_x) * a.TW;
-                int src = 0, chunk_base = 0;
-                for (int kb = 0; kb < a.nkb; ++kb) {
-                    const int gchunk = kb / a.ntaps, tap = kb - gchunk * a.ntaps;
-                    while (gchunk >= a.chunk_end[src]) { chunk_base = a.chunk_end[src]; ++src; }
-                    const int dy = a.ntaps == 9 ? tap / 3 - 1 : 0, dx = a.ntaps == 9 ? tap % 3 - 1 : 0;
-                    const int simg = a.src_img[src] ? a.src_img[src][img] : img;
-                    mbar_wait(bar_empty + 8u * s, ph ^ 1u);
-                    if (tr && tn < TRACE_N) tr[tn * 8 + 0] = clock64();
-                    mbar_expect_tx(bar_full + 8u * s, stage_bytes);
-                    const uint32_t st = smem_base + s * stage_bytes;
-                    const int c0 = (gchunk - chunk_base) * 64;
-                    tma_load_5d(&a.amap[src], bar_full + 8u * s, st, c0, x0 + dx, y0 + dy, simg, 0);
-                    tma_load_5d(&a.amap[src], bar_full + 8u * s, st + TC_A_BYTES, c0, x0 + dx, y0 + dy, simg, 1);
-                    tma_load_3d(&a.bmap_half, bar_full + 8u * s, st + 2u * TC_A_BYTES, 0, brow, kb);
-                    tma_load_3d(&a.bmap_half, bar_full + 8u * s, st + 2u * TC_A_BYTES + bh_bytes, 0, brow, a.nkb + kb);
-                    if (tr && tn < TRACE_N) { tr[tn * 8 + 1] = clock64(); ++tn; }
-                    if (++s == (uint32_t)a.stages) { s = 0; ph ^= 1u; }
-                }
-            }
-        }
-    } else if (warp == 1) {
-        const bool one = elect_one_sync();
-        if (one && rank == 1) {
-            // ===================== rank 1: forward "stage landed" to the leader =====================
-            uint32_t s = 0, ph = 0;
-            long long *tr = (a.trace && blockIdx.x == 1) ? a.trace : nullptr;
-            int tn = 0;
-            for (int pr = pair0; pr < n_pairs; pr += pair_step)
-                for (int kb = 0; kb < a.nkb; ++kb) {
-                    mbar_wait(bar_full + 8u * s, ph);
-                    if (tr && tn < TRACE_N) { tr[tn * 8 + 6] = clock64(); ++tn; }
-                    mbar_arrive_remote(bar_pfull + 8u * s, 0u);
-                    if (++s == (uint32_t)a.stages) { s = 0; ph ^= 1u; }
-                }
-        } else if (one) {
-            // ===================== leader: MMA issuer for the pair =====================
-            const uint32_t idesc = umma_idesc(2 * TC_BLOCK_M, a.npad);
-            uint32_t s = 0, ph = 0;
-            int it = 0;
-            long long *tr = (a.trace && blockIdx.x == 0) ? a.trace : nullptr;
-            int tn = 0;
-            for (int pr = pair0; pr < n_pairs; pr += pair_step, ++it) {
-                const uint32_t ai = (uint32_t)(it & 1), aph = (uint32_t)((it >> 1) & 1);
-                mbar_wait(bar_aempty + 8u * ai, aph ^ 1u);  // both CTAs' epilogues of pair it-2 have drained this accumulator
-                tc_fence_after();
-                const uint32_t acc = tmem_base + ai * 256u;
-                for (int kb = 0; kb < a.nkb; ++kb) {
-                    if (tr && tn < TRACE_N) tr[tn * 8 + 2] = clock64();
-                    mbar_wait(bar_full + 8u * s, ph);
-                    if (tr && tn < TRACE_N) tr[tn * 8 + 3] = clock64();
-                    mbar_wait(bar_pfull + 8u * s, ph);
-                    tc_fence_after();
-                    if (tr && tn < TRACE_N) tr[tn * 8 + 5] = clock64();
-                    const uint32_t st = smem_base + s * stage_bytes;
-                    const uint32_t a_hi = st, a_lo = st + TC_A_BYTES, b_hi = st + 2u * TC_A_BYTES, b_lo = b_hi + bh_bytes;
-#pragma unroll
-                    for (int k = 0; k < 4; ++k) {
-                        const uint64_t dah = umma_desc(umma_desc_lo(a_hi) + 2u * k, UMMA_HI_1024), dal = umma_desc(umma_desc_lo(a_lo) + 2u * k, UMMA_HI_1024);
-                        const uint64_t dbh = umma_desc(umma_desc_lo(b_hi) + 2u * k, UMMA_HI_1024), dbl = umma_desc(umma_desc_lo(b_lo) + 2u * k, UMMA_HI_1024);
-                        umma_bf16_pair(acc, dal, dbh, idesc, (kb | k) != 0 ? 1u : 0u);
-                        umma_bf16_pair(acc, dah, dbl, idesc, 1u);
-                        umma_bf16_pair(acc, dah, dbh, idesc, 1u);
-                    }
-                    umma_commit_pair(bar_empty + 8u * s);
-                    if (tr && tn < TRACE_N) { tr[tn * 8 + 4] = clock64(); ++tn; }
-                    if (++s == (uint32_t)a.stages) { s = 0; ph ^= 1u; }
-                }
-                umma_commit_pair(bar_afull + 8u * ai);
-            }
-        }
-    } else {
-        // ===================== epilogue (both CTAs): own 128 accumulator rows = own pixel tile =====================
-        const int quad = warp & 3;
-        const int m = quad * 32 + lane;
-        int it = 0;
-        for (int pr = pair0; pr < n_pairs; pr += pair_step, ++it) {
-            const uint32_t ai = (uint32_t)(it & 1), aph = (uint32_t)((it >> 1) & 1);
-            const int tile_raw = 2 * pr + (int)rank;
-            const int tile = min(tile_raw, n_tiles - 1);
-            const int img = tile / tiles_per_img, trem = tile - img * tiles_per_img;
-            const int y0 = (trem / a.tiles_x) * a.TH, x0 = (trem % a.tiles_x) * a.TW;
-            const int y = y0 + m / a.TW, x = x0 + m % a.TW;
-            const bool valid = (tile_raw < n_tiles) && (y < a.H) && (x < a.W);
-            const size_t pix = ((size_t)img * a.H + (valid ? y : 0)) * a.W + (valid ? x : 0);
-            mbar_wait_backoff(bar_afull + 8u * ai, aph);
-            tc_fence_after();
-            const uint32_t taddr = tmem_base + ai * 256u + ((uint32_t)(quad * 32) << 16);
-            for (int n0 = 0; n0 < a.npad; n0 += 32) {
-                uint32_t raw[32];
-                if (a.npad - n0 >= 32) {
-                    tmem_ld32(taddr + (uint32_t)n0, raw);
-                } else {
-                    uint32_t r16[16];
-                    asm volatile("tcgen05.ld.sync.aligned.32x32b.x16.b32"
-                                 "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-                                 : "=r"(r16[0]), "=r"(r16[1]), "=r"(r16[2]), "=r"(r16[3]), "=r"(r16[4]), "=r"(r16[5]),
-                                   "=r"(r16[6]), "=r"(r16[7]), "=r"(r16[8]), "=r"(r16[9]), "=r"(r16[10]), "=r"(r16[11]),
-                                   "=r"(r16[12]), "=r"(r16[13]), "=r"(r16[14]), "=r"(r16[15])
-                                 : "r"(taddr + (uint32_t)n0));
-                    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-                    for (int j = 0; j < 16; ++j) { raw[j] = r16[j]; raw[16 + j] = 0u; }
-                }
-                if (valid) epilogue_chunk(a, raw, n0, pix, img, y, x);
-                __syncwarp();
-            }
-            tc_fence_before();                                       // this warp's TMEM reads are done: release the accumulator
-            __syncwarp();
-            if (lane == 0) mbar_arrive_remote(bar_aempty + 8u * ai, 0u);   // leader's barrier (for the leader: its own)
-        }
+__global__ void __launch_bounds__(TC_THREADS, 1) k_gru_chain(const ConvTCArgs *__restrict__ args, int nphase, int stages,
+                                                             unsigned int *ctr)
+{
+    const TcSmem m = tc_smem_layout(128, stages);
+    tc_init_barriers(m);
+    TcRing ring;
+    for (int p = 0; p < nphase; ++p) {
+        if (p & 1) conv_tiles<64>(args[p], blockIdx.x, gridDim.x, m, ring);
+        else conv_tiles<128>(args[p], blockIdx.x, gridDim.x, m, ring);
+        grid_barrier(ctr, (unsigned int)(p + 1) * gridDim.x);
     }
-
-    tc_fence_before();
-    pair_sync();                     // nobody leaves while the peer may still read this CTA's operands or arrive on its barriers
-    if (warp == 1) { tc_fence_after(); tmem_dealloc_pair(tmem_base, 512); }
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -553,48 +255,8 @@ static int make_bmap(const void *w, int npad, int nkb, int box_rows, CUtensorMap
     return ESR_OK;
 }
 
-// Output side: 32 channels x (BW x BH = 32 pixels) per box, 64-byte rows with the 64-byte swizzle (conflict-free 16-byte
-// shared-memory stores by 32 lanes that own one pixel each).
-int tc_make_omap(const SplitTensor &t, int BW, int BH, CUtensorMap *out)
-{
-    PFN_tmapEncodeTiled enc = get_encode();
-    if (!enc) { set_error("cuTensorMapEncodeTiled unavailable"); return ESR_ECUDA; }
-    const cuuint64_t C = t.C, W = t.W, H = t.H, N = t.n_img;
-    cuuint64_t gdim[5] = {C, W, H, N, 2};
-    cuuint64_t gstr[4] = {C * 2, W * C * 2, H * W * C * 2, (cuuint64_t)t.plane() * 2};
-    cuuint32_t box[5] = {32, (cuuint32_t)BW, (cuuint32_t)BH, 1, 1};
-    cuuint32_t estr[5] = {1, 1, 1, 1, 1};
-    CUresult r = enc(out, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 5, t.base, gdim, gstr, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                     CU_TENSOR_MAP_SWIZZLE_64B, CU_TENSOR_MAP_L2_PROMOTION_NONE, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_SUCCESS) { set_error("cuTensorMapEncodeTiled(out) failed: %d (C=%d W=%d H=%d N=%d)", (int)r, t.C, t.W, t.H, t.n_img); return ESR_ECUDA; }
-    return ESR_OK;
-}
-int tc_make_omap_f32(float *base, int n_img, int H_, int W_, int C_, int BW, int BH, CUtensorMap *out)
-{
-    PFN_tmapEncodeTiled enc = get_encode();
-    if (!enc) { set_error("cuTensorMapEncodeTiled unavailable"); return ESR_ECUDA; }
-    const cuuint64_t C = C_, W = W_, H = H_, N = n_img;
-    cuuint64_t gdim[5] = {C, W, H, N, 1};
-    cuuint64_t gstr[4] = {C * 4, W * C * 4, H * W * C * 4, N * H * W * C * 4};
-    cuuint32_t box[5] = {32, (cuuint32_t)BW, (cuuint32_t)BH, 1, 1};
-    cuuint32_t estr[5] = {1, 1, 1, 1, 1};
-    CUresult r = enc(out, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 5, base, gdim, gstr, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                     CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_NONE, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_SUCCESS) { set_error("cuTensorMapEncodeTiled(out f32) failed: %d (C=%d W=%d H=%d N=%d)", (int)r, C_, W_, H_, n_img); return ESR_ECUDA; }
-    return ESR_OK;
-}
 int tc_make_amap(const SplitTensor &t, int BW, int BH, CUtensorMap *out) { return make_amap(t, BW, BH, out); }
 int tc_make_bmap(const void *w, int npad, int nkb, int box_rows, CUtensorMap *out) { return make_bmap(w, npad, nkb, box_rows, out); }
-
-static size_t tc_smem_bytes(int npad, int stages)
-{
-    return 1024 + (size_t)stages * (2 * TC_A_BYTES + 2 * (size_t)npad * 128) + 16 * (size_t)stages + 64;
-}
-
-static size_t tc_pair_smem_bytes(int npad, int stages)
-{
-    return 1024 + (size_t)stages * (2 * TC_A_BYTES + (size_t)npad * 128) + 24 * (size_t)stages + 96;
-}
 
 int conv_tc_prepare(const ConvTCDesc &d, ConvTCArgs *args)
 {
@@ -605,46 +267,15 @@ int conv_tc_prepare(const ConvTCDesc &d, ConvTCArgs *args)
     const int H = d.src[0].H, W = d.src[0].W;
     int chunks = 0;
     // tile shape: 128 pixels; prefer wide tiles, but do not waste more than half a tile on narrow images
-    int TW = W >= 24 ? 32 : (W >= 12 ? 16 : 8);
-    int TH = TC_BLOCK_M / TW;
-    // The halo-reuse + weight-multicast kernel (tc_conv3.cu: 8 x 16 tiles, 16 x 18 halo boxes) is opt-in (ESR_TC_V3=1):
-    // measured on B200 it is 5-50 % SLOWER than this kernel with two co-resident CTAs per SM (profiles/r1_notes.md) --
-    // the main loop turned out to be latency / shared-memory-port bound, not L2-bandwidth bound.
-    static const bool use_v3 = getenv("ESR_TC_V3") != nullptr;
-    const int npad_ = tc_npad(d.cout);
-    int a_st = 0, b_st = 0;
-    static const int v3_min_n = getenv("ESR_TC_V3_MIN_N") ? atoi(getenv("ESR_TC_V3_MIN_N")) : 0;   // restrict the experiment to wide layers
-    const bool v3 = d.ntaps == 9 && use_v3 && npad_ >= v3_min_n && conv_tc3_plan(npad_, &a_st, &b_st);
-    int BW = TW, BH = TH;
-    if (v3) { TW = 8; TH = 16; BW = 16; BH = 18; }
-    // multi-wave 3x3 layers: persistent halo-reuse kernel (tc_conv_halo.cu; ESR_TC_NO_HALO=1 keeps k_conv_tc_persist)
-    static const bool no_halo = getenv("ESR_TC_NO_HALO") != nullptr;
-    int h_as = 0, h_bs = 0;
-    // epilogue through shared memory + TMA stores (ESR_TC_NO_OUT_TMA=1: direct 16-byte stores): plain split outputs only
-    static const bool no_out_tma = getenv("ESR_TC_NO_OUT_TMA") != nullptr;
-    int out_tma = 0, stg_bufs = 0;
-    if (!no_out_tma && d.epi_mode == EPI_STD) {
-        if (d.out.base && !d.out_f32 && d.cout % 32 == 0 && d.out.C % 8 == 0 && d.out_coff % 8 == 0) out_tma = 1;
-        else if (!d.out.base && d.out_f32 && !d.out_f32_nchw && d.out_f32_C % 4 == 0 && ((uintptr_t)d.out_f32 & 15) == 0) out_tma = 2;
-    }
-    bool halo = !v3 && !no_halo && d.ntaps == 9 && getenv("ESR_TC_PAIR") == nullptr &&
-                d.n_img * ((W + 7) / 8) * ((H + 15) / 16) > dev_info().sm_count;
-    if (halo && out_tma) {
-        if (conv_tc_halo_plan(npad_, 2, &h_as, &h_bs)) stg_bufs = 2;
-        else if (conv_tc_halo_plan(npad_, 1, &h_as, &h_bs)) stg_bufs = 1;
-        else out_tma = 0;
-    }
-    if (halo && !out_tma) halo = conv_tc_halo_plan(npad_, 0, &h_as, &h_bs);
-    const int out_tma_req = out_tma;                              // eligibility of the output, whichever kernel takes the layer
-    if (!halo) out_tma = 0;                                       // (decided below for the persistent kernel; the one-tile kernel keeps direct stores)
-    if (halo) { TW = 8; TH = 16; BW = 10; BH = 18; }
+    const int TW = W >= 24 ? 32 : (W >= 12 ? 16 : 8);
+    const int TH = TC_BLOCK_M / TW;
     for (int s = 0; s < d.n_src; ++s) {
         const SplitTensor &t = d.src[s];
         ESR_REQUIRE(t.base && t.C % 64 == 0 && t.H == H && t.W == W, "conv_tc: source %d has C=%d H=%d W=%d", s, t.C, t.H, t.W);
         chunks += t.C / 64;
         a.chunk_end[s] = chunks;
         a.src_img[s] = d.src_img[s];
-        int rc = make_amap(t, BW, BH, &a.amap[s]);
+        int rc = make_amap(t, TW, TH, &a.amap[s]);
         if (rc) return rc;
     }
     for (int s = d.n_src; s < TC_MAX_SRC; ++s) a.chunk_end[s] = 1 << 30;
@@ -653,55 +284,21 @@ int conv_tc_prepare(const ConvTCDesc &d, ConvTCArgs *args)
     ESR_REQUIRE(a.npad <= 256, "conv_tc: cout=%d too large", d.cout);
     int rc = make_bmap(d.wpacked, a.npad, a.nkb, a.npad, &a.bmap);
     if (rc) return rc;
-    a.kernel_ver = v3 ? 3 : (halo ? 4 : 1);
-    // stacked weights: for N <= 128 the two products that share A_hi run as ONE MMA over [B_hi; B_lo] (N' = 2 N <= 256): 8 instead of 12
-    // MMAs per K-block and A_hi is read from shared memory once instead of twice (the kernels are shared-memory-port bound)
-    { static const bool no_stack = getenv("ESR_TC_NO_STACK") != nullptr; a.stack = (!v3 && !no_stack && a.npad <= 128) ? 1 : 0; }
-    { static const int diag = getenv("ESR_TC_DIAG") ? atoi(getenv("ESR_TC_DIAG")) : 0; a.diag = diag; }
-    a.cluster = 1; a.a_stages = a_st;
     a.H = H; a.W = W; a.TW = TW; a.TH = TH;
     a.tiles_x = (W + TW - 1) / TW; a.tiles_y = (H + TH - 1) / TH; a.n_img = d.n_img;
-    // Pipeline depth.  Grids of more than one wave keep two CTAs resident per SM (<= half the shared memory each) so that
-    // one CTA's prologue / epilogue overlaps the other's main loop; single-wave grids take all the stages that fit.
+    // Pipeline depth: all the stages that fit.  Grids of more than one wave keep two persistent CTAs resident per SM where the
+    // registers allow it (npad <= 64, see the kernel's launch bounds) and each fits in half the shared memory.
     const size_t smem_cap = (size_t)dev_info().max_smem_optin;
     const int n_tiles = d.n_img * a.tiles_x * a.tiles_y;
     int stages = 6;
     while (stages > 2 && tc_smem_bytes(a.npad, stages) > smem_cap) --stages;
-    // multi-wave grids of layers with N >= 64: persistent CTAs (one per SM, all the stages that fit) with two TMEM accumulators
-    static const int persist_min_n = getenv("ESR_TC_NO_PERSIST") ? 1 << 30 : (getenv("ESR_TC_PERSIST_MIN_N") ? atoi(getenv("ESR_TC_PERSIST_MIN_N")) : 64);   // measured: 129 -> 3.196 ms, 64 -> 3.159 ms, 16 -> 3.165 ms per cfg2 step
-    a.persist = (!v3 && !halo && a.npad >= persist_min_n && n_tiles > dev_info().sm_count) ? 1 : 0;
-    if (a.persist && out_tma_req == 1 && 32 % TW == 0 && getenv("ESR_TC_PAIR") == nullptr) {
-        int st2 = stages;                                         // staged TMA-store epilogue also here: 32 KB of staging beside the ring
-        while (st2 > 2 && tc_smem_bytes(a.npad, st2) + 64 + 4 * 2 * 4096 > smem_cap) --st2;
-        if (tc_smem_bytes(a.npad, st2) + 64 + 4 * 2 * 4096 <= smem_cap) { stages = st2; out_tma = 1; stg_bufs = 2; }
-    }
-    if (n_tiles > dev_info().sm_count && !a.persist) {
+    if (n_tiles > dev_info().sm_count && a.npad <= 64) {
         int s2 = stages;
         while (s2 > 2 && 2 * (tc_smem_bytes(a.npad, s2) + 1024) > smem_cap) --s2;
         if (2 * (tc_smem_bytes(a.npad, s2) + 1024) <= smem_cap) stages = s2;
     }
-    { static const int cap = getenv("ESR_TC_STAGES") ? atoi(getenv("ESR_TC_STAGES")) : 0; if (cap >= 2 && stages > cap) stages = cap; }   // measurement aid
     if (stages > a.nkb) stages = a.nkb < 2 ? 2 : a.nkb;
     a.stages = stages;
-    // CTA pairs (tcgen05 cta_group::2) for the persistent layers: half the weight bytes per CTA -> deeper pipeline (ESR_TC_NO_PAIR=1: off)
-    static const bool no_pair = getenv("ESR_TC_PAIR") == nullptr;       // opt-in: measured slower than the single-CTA kernel (profiles/r2_notes.md)
-    a.pair = 0;
-    if (a.persist && !no_pair && n_tiles >= 2 && dev_info().sm_count >= 2) {
-        int sp = 8;
-        while (sp > 2 && tc_pair_smem_bytes(a.npad, sp) > smem_cap) --sp;
-        if (tc_pair_smem_bytes(a.npad, sp) <= smem_cap) {
-            if (sp > a.nkb) sp = a.nkb < 2 ? 2 : a.nkb;
-            a.pair = 1; a.stages = sp;
-            if ((rc = make_bmap(d.wpacked, a.npad, a.nkb, a.npad / 2, &a.bmap_half))) return rc;
-        }
-    }
-    if (halo) { a.a_stages = h_as; a.stages = h_bs; }
-    if (v3) {
-        static const bool no_mc = getenv("ESR_TC_NO_MULTICAST") != nullptr;
-        a.stages = b_st;
-        a.cluster = (!no_mc && n_tiles >= 2) ? 2 : 1;
-        if (a.cluster == 2 && (rc = make_bmap(d.wpacked, a.npad, a.nkb, a.npad / 2, &a.bmap_half))) return rc;
-    }
     a.bias = d.bias;
     a.act = d.act; a.act_from = d.act_from; a.res_mode = d.res_mode; a.epi_mode = d.epi_mode;
     if (d.res_mode != RES_NONE) {
@@ -712,14 +309,6 @@ int conv_tc_prepare(const ConvTCDesc &d, ConvTCArgs *args)
         ESR_REQUIRE(d.out.H == H && d.out.W == W && d.out.n_img >= d.n_img && d.out.C % 8 == 0 && d.out_coff % 8 == 0,
                     "conv_tc: bad split output");
         a.out = d.out.base; a.out_plane = d.out.plane(); a.out_C = d.out.C; a.out_coff = d.out_coff;
-        if (out_tma == 1) {
-            a.out_tma = 1; a.stg_bufs = stg_bufs;
-            if ((rc = tc_make_omap(d.out, TW, 32 / TW, &a.omap))) return rc;
-        }
-    }
-    if (out_tma == 2) {
-        a.out_tma = 2; a.stg_bufs = stg_bufs;
-        if ((rc = tc_make_omap_f32(d.out_f32, d.n_img, H, W, d.out_f32_C, TW, 32 / TW, &a.omap))) return rc;
     }
     a.out_f32 = d.out_f32; a.out_f32_C = d.out_f32_C; a.out_f32_nchw = d.out_f32_nchw;
     if (d.epi_mode != EPI_STD) {
@@ -732,92 +321,107 @@ int conv_tc_prepare(const ConvTCDesc &d, ConvTCArgs *args)
     return ESR_OK;
 }
 
-int conv_tc_launch(const ConvTCArgs &a, cudaStream_t st)
+// one instantiation per padded width (multiples of 16 up to 256): the accumulator is a register array of npad / 2 floats
+template <int NP>
+static int launch_np(const ConvTCArgs &a, cudaStream_t st)
 {
-    if (a.kernel_ver == 3) return conv_tc3_launch(a, st);
-    if (a.kernel_ver == 4) return conv_tc_halo_launch(a, st);
     static int max_set = 0;
-    const size_t smem = tc_smem_bytes(a.npad, a.stages);
-    if (!(a.persist && a.pair) && (int)smem > max_set) {
-        ESR_CUDA_CHECK(cudaFuncSetAttribute(k_conv_tc, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    const size_t smem = tc_smem_bytes(NP, a.stages);
+    if ((int)smem > max_set) {
+        ESR_CUDA_CHECK(cudaFuncSetAttribute(k_conv_tc<NP>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         max_set = (int)smem;
     }
-    const unsigned grid = (unsigned)(a.n_img * a.tiles_x * a.tiles_y);
-    // wide layers (one CTA per SM) on multi-wave grids: persistent CTAs with two TMEM accumulators (ESR_TC_NO_PERSIST=1: off)
-    if (a.persist && a.pair) {
-        static int max_set_q = 0;
-        const size_t smem_q = tc_pair_smem_bytes(a.npad, a.stages);
-        if ((int)smem_q > max_set_q) {
-            ESR_CUDA_CHECK(cudaFuncSetAttribute(k_conv_tc_pair, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_q));
-            max_set_q = (int)smem_q;
-        }
-        const int n_pairs = ((int)grid + 1) / 2;
-        const unsigned g2 = 2u * (unsigned)min(n_pairs, dev_info().sm_count / 2);
-        static const char *trace_path = getenv("ESR_TC_TRACE");          // measurement aid, see the persistent kernel below
-        if (trace_path) {
-            static long long *dbuf = nullptr;
-            int want_n = 0, want_k = 0; char path[512] = {0};
-            if (sscanf(trace_path, "%511[^:]:%d:%d", path, &want_n, &want_k) == 3 && want_n == a.npad && want_k == a.nkb) {
-                if (!dbuf) cudaMalloc(&dbuf, sizeof(long long) * 8 * TRACE_N);
-                cudaMemsetAsync(dbuf, 0, sizeof(long long) * 8 * TRACE_N, st);
-                ConvTCArgs b = a; b.trace = dbuf;
-                k_conv_tc_pair<<<g2, TC_THREADS, smem_q, st>>>(b);
-                cudaStreamSynchronize(st);
-                static long long host[8 * TRACE_N];
-                cudaMemcpy(host, dbuf, sizeof(host), cudaMemcpyDeviceToHost);
-                FILE *f = fopen(path, "w");
-                if (f) {
-                    fprintf(f, "# PAIR npad=%d nkb=%d stages=%d tiles=%d; per K-block: prod_after_empty_wait, prod_after_issue, mma_before_full_wait, mma_after_full_wait, mma_after_commit, mma_after_pfull_wait, relay_after_full_wait(rank1 clock)\n", a.npad, a.nkb, a.stages, (int)grid);
-                    for (int i = 0; i < TRACE_N; ++i) { for (int c = 0; c < 7; ++c) fprintf(f, "%lld%c", host[i * 8 + c], c == 6 ? '\n' : ','); }
-                    fclose(f);
-                }
-                ESR_LAUNCH_CHECK();
-                return ESR_OK;
-            }
-        }
-        k_conv_tc_pair<<<g2, TC_THREADS, smem_q, st>>>(a);
-        ESR_LAUNCH_CHECK();
-        return ESR_OK;
-    }
-    if (a.persist) {
-        static const char *trace_path = getenv("ESR_TC_TRACE");          // measurement aid: "<file>:<npad>:<nkb>" traces launches of that shape
-        if (trace_path) {
-            static long long *dbuf = nullptr;
-            int want_n = 0, want_k = 0; char path[512] = {0};
-            if (sscanf(trace_path, "%511[^:]:%d:%d", path, &want_n, &want_k) == 3 && want_n == a.npad && want_k == a.nkb) {
-                if (!dbuf) cudaMalloc(&dbuf, sizeof(long long) * 8 * TRACE_N);
-                cudaMemsetAsync(dbuf, 0, sizeof(long long) * 8 * TRACE_N, st);
-                ConvTCArgs b = a; b.trace = dbuf;
-                static int max_set_t = 0;
-                const size_t smem_t = smem + 64 + (a.out_tma ? 4 * 2 * 4096 : 0);
-                if ((int)smem_t > max_set_t) { cudaFuncSetAttribute(k_conv_tc_persist, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_t); max_set_t = (int)smem_t; }
-                k_conv_tc_persist<<<(unsigned)dev_info().sm_count, TC_THREADS, smem_t, st>>>(b);
-                cudaStreamSynchronize(st);
-                static long long host[8 * TRACE_N];
-                cudaMemcpy(host, dbuf, sizeof(host), cudaMemcpyDeviceToHost);
-                FILE *f = fopen(path, "w");
-                if (f) {
-                    fprintf(f, "# npad=%d nkb=%d stages=%d tiles=%d; per K-block: prod_after_empty_wait, prod_after_issue, mma_before_full_wait, mma_after_full_wait, mma_after_commit; per tile (same rows, by tile index): epi_start, epi_end\n", a.npad, a.nkb, a.stages, a.n_img * a.tiles_x * a.tiles_y);
-                    for (int i = 0; i < TRACE_N; ++i) { for (int c = 0; c < 7; ++c) fprintf(f, "%lld%c", host[i * 8 + c], c == 6 ? '\n' : ','); }
-                    fclose(f);
-                }
-                ESR_LAUNCH_CHECK();
-                return ESR_OK;
-            }
-        }
-        static int max_set_p = 0;
-        const size_t smem_p = smem + 64 + (a.out_tma ? 4 * 2 * 4096 : 0);
-        if ((int)smem_p > max_set_p) {
-            ESR_CUDA_CHECK(cudaFuncSetAttribute(k_conv_tc_persist, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_p));
-            max_set_p = (int)smem_p;
-        }
-        ESR_CUDA_CHECK(launch_pdl(k_conv_tc_persist, dim3((unsigned)dev_info().sm_count), dim3(TC_THREADS), smem_p, st, a));
-        esr::count_launch();
-        return ESR_OK;
-    }
-    ESR_CUDA_CHECK(launch_pdl(k_conv_tc, dim3(grid), dim3(TC_THREADS), smem, st, a));
+    int per_sm = 0;
+    ESR_CUDA_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_conv_tc<NP>, TC_THREADS, smem));
+    const int n_tiles = a.n_img * a.tiles_x * a.tiles_y;
+    const unsigned grid = (unsigned)std::max(1, std::min(n_tiles, std::max(per_sm, 1) * dev_info().sm_count));
+    ESR_CUDA_CHECK(launch_pdl(k_conv_tc<NP>, dim3(grid), dim3(TC_THREADS), smem, st, a));
     esr::count_launch();
     return ESR_OK;
+}
+
+int conv_tc_launch(const ConvTCArgs &a, cudaStream_t st)
+{
+    switch (a.npad) {
+    case 16: return launch_np<16>(a, st);
+    case 32: return launch_np<32>(a, st);
+    case 48: return launch_np<48>(a, st);
+    case 64: return launch_np<64>(a, st);
+    case 80: return launch_np<80>(a, st);
+    case 96: return launch_np<96>(a, st);
+    case 112: return launch_np<112>(a, st);
+    case 128: return launch_np<128>(a, st);
+    case 144: return launch_np<144>(a, st);
+    case 160: return launch_np<160>(a, st);
+    case 176: return launch_np<176>(a, st);
+    case 192: return launch_np<192>(a, st);
+    case 208: return launch_np<208>(a, st);
+    case 224: return launch_np<224>(a, st);
+    case 240: return launch_np<240>(a, st);
+    case 256: return launch_np<256>(a, st);
+    }
+    set_error("conv_tc: npad=%d", a.npad);
+    return ESR_EINVAL;
+}
+
+struct GruChainPlan { ConvTCArgs *args = nullptr; unsigned int *ctr = nullptr; int nphase = 0, stages = 2; unsigned grid = 0; size_t smem = 0; };
+
+int gru_chain_prepare(const std::vector<ConvTCArgs> &zr, const std::vector<ConvTCArgs> &go, void **plan_out)
+{
+    ESR_REQUIRE(!zr.empty() && zr.size() == go.size(), "gru_chain: %zu / %zu steps", zr.size(), go.size());
+    GruChainPlan *p = new GruChainPlan();
+    std::vector<ConvTCArgs> ph;
+    for (size_t g = 0; g < zr.size(); ++g) {
+        if (zr[g].npad != 128 || go[g].npad != 64 || zr[g].epi_mode != EPI_GRU_ZR || go[g].epi_mode != EPI_GRU_OUT) {
+            delete p; set_error("gru_chain: unexpected gate layers"); return ESR_EINVAL;
+        }
+        ph.push_back(zr[g]); ph.push_back(go[g]);
+    }
+    p->nphase = (int)ph.size();
+    const size_t cap = (size_t)dev_info().max_smem_optin;
+    int stages = 6;
+    while (stages > 2 && tc_smem_bytes(128, stages) > cap) --stages;
+    p->stages = stages;
+    p->smem = tc_smem_bytes(128, stages);
+    cudaError_t e = cudaFuncSetAttribute(k_gru_chain, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)p->smem);
+    int per_sm = 0;
+    if (e == cudaSuccess) e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_gru_chain, TC_THREADS, p->smem);
+    if (e == cudaSuccess && per_sm < 1) e = cudaErrorInvalidConfiguration;
+    const int n_tiles = zr[0].n_img * zr[0].tiles_x * zr[0].tiles_y;
+    p->grid = (unsigned)std::min(n_tiles, per_sm * dev_info().sm_count);      // all CTAs co-resident (cooperative launch)
+    if (e == cudaSuccess) e = cudaMalloc(&p->args, sizeof(ConvTCArgs) * ph.size());
+    if (e == cudaSuccess) e = cudaMalloc(&p->ctr, 256);
+    if (e == cudaSuccess) e = cudaMemcpy(p->args, ph.data(), sizeof(ConvTCArgs) * ph.size(), cudaMemcpyHostToDevice);
+    if (e != cudaSuccess) {
+        set_error("gru_chain: %s", cudaGetErrorString(e));
+        cudaFree(p->args); cudaFree(p->ctr); delete p;
+        return ESR_ECUDA;
+    }
+    *plan_out = p;
+    return ESR_OK;
+}
+
+int gru_chain_launch(void *plan, cudaStream_t st)
+{
+    GruChainPlan *p = (GruChainPlan *)plan;
+    ESR_CUDA_CHECK(cudaMemsetAsync(p->ctr, 0, sizeof(unsigned int), st));
+    cudaLaunchConfig_t cfg{};
+    cfg.gridDim = dim3(p->grid); cfg.blockDim = dim3(TC_THREADS); cfg.dynamicSmemBytes = p->smem; cfg.stream = st;
+    cudaLaunchAttribute at[1];
+    at[0].id = cudaLaunchAttributeCooperative;
+    at[0].val.cooperative = 1;
+    cfg.attrs = at; cfg.numAttrs = 1;
+    ESR_CUDA_CHECK(cudaLaunchKernelEx(&cfg, k_gru_chain, (const ConvTCArgs *)p->args, p->nphase, p->stages, p->ctr));
+    esr::count_launch();
+    return ESR_OK;
+}
+
+void gru_chain_destroy(void *plan)
+{
+    GruChainPlan *p = (GruChainPlan *)plan;
+    if (!p) return;
+    cudaFree(p->args); cudaFree(p->ctr);
+    delete p;
 }
 
 // ------------------------------------------------------------------------------------------------

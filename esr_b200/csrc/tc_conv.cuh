@@ -1,12 +1,10 @@
-// tc_conv.cuh -- interface of the tcgen05 implicit-GEMM convolution (see tc_conv.cu).
+// tc_conv.cuh -- interface of the wgmma implicit-GEMM convolution (see tc_conv.cu).
 #pragma once
 #include "common.cuh"
 #include <cuda.h>   // CUtensorMap (types only; the driver entry point is resolved at run time)
+#include <vector>
 
 namespace esr {
-constexpr int TRACE_N = 512;                 // K-blocks / tiles recorded by the ESR_TC_TRACE measurement aid
-
-
 enum Act : int { ACT_NONE = 0, ACT_RELU = 1, ACT_SIGMOID = 2, ACT_TANH = 3 };
 enum EpiMode : int { EPI_STD = 0, EPI_GRU_ZR = 1, EPI_GRU_OUT = 2 };
 enum ResMode : int { RES_NONE = 0, RES_PRE_ACT = 1, RES_POST_ACT = 2 };
@@ -26,28 +24,11 @@ constexpr int TC_MAX_SRC = 3;
 struct ConvTCArgs {
     CUtensorMap amap[TC_MAX_SRC];   // 5-D maps over the source split tensors (C, W, H, img, plane), box (64, TW, TH, 1, 1)
     CUtensorMap bmap;               // 3-D map over packed weights (64, npad, 2*nkb), box (64, npad, 1)
-    // The argument block must stay <= 1024 bytes: above that every launch of these kernels measured ~4 us slower (the store-side map
-    // added as its own member made it 1088 bytes and cost 19 launches x 4 us per step).  The two maps below are never used together.
-    union {
-        CUtensorMap bmap_half;      // same tensor, box (64, npad/2, 1): the half a CTA multicasts in a 2-CTA cluster (pair / v3 kernels)
-        CUtensorMap omap;           // out_tma (halo kernel): 5-D map over the OUTPUT (C, W, H, img, plane), box (32, TW, 32 / TW, 1, 1)
-    };
-    int out_tma;                    // 1: the epilogue stages each warp's 32 pixels x 32 channels in shared memory and stores them with TMA (split output);
-                                    // 2: same for the fp32 NHWC output (omap: (C, W, H, img, 1) fp32, SWIZZLE_128B)
-    int stg_bufs;                   // staging buffers per epilogue warp (2, or 1 when shared memory is short)
-    int kernel_ver;                 // 1: tc_conv.cu (tap-shifted tiles), 3: tc_conv3.cu (halo reuse + weight multicast), 4: tc_conv_halo.cu
-    int stack;                      // 1: [B_hi; B_lo] stacked along N -- two MMAs per K-step (A_hi x [B_hi;B_lo], A_lo x B_hi) instead of three
-    int pair;                       // 1 (with persist): k_conv_tc_pair, two-CTA clusters issuing tcgen05.mma.cta_group::2
-    int persist;                    // 1: k_conv_tc_persist (one CTA per SM walks the tiles, two TMEM accumulators)
-    int a_stages, cluster;          // v3 only: halo ring depth, cluster size (1 or 2)
     const int *src_img[TC_MAX_SRC]; // output image -> source image (nullptr = identity)
     int chunk_end[TC_MAX_SRC];      // cumulative number of 64-channel chunks after source s
     int n_src, ntaps, nkb, npad, cout;
     int H, W, TW, TH, tiles_x, tiles_y, n_img;
     int stages;
-    int trace_cta;                  // the CTA whose stamps are recorded (ESR_TC_TRACE_CTA, default 0)
-    long long *trace;               // measurement aid (ESR_TC_TRACE): clock64 stamps of CTA 0's producer / MMA / epilogue threads
-    int diag;                       // measurement aid (ESR_TC_DIAG): bit 0 = do not load the lo plane of B, bit 1 = not the lo plane of A (wrong results)
     // epilogue
     const float *bias;              // [npad]
     int act, act_from, res_mode, epi_mode;
@@ -89,17 +70,13 @@ static inline size_t tc_packed_weight_bytes(int cout, int cin_total, int ntaps)
 // Builds tensor maps + launch geometry.  H, W taken from src[0].
 int conv_tc_prepare(const ConvTCDesc &d, ConvTCArgs *args);
 int conv_tc_launch(const ConvTCArgs &args, cudaStream_t st);
-// tensor-map builders (shared with gru_chain.cu)
+// the ConvGRU recurrence as one cooperative launch over the prepared gate layers of every step (EPI_GRU_ZR / EPI_GRU_OUT)
+int gru_chain_prepare(const std::vector<ConvTCArgs> &zr, const std::vector<ConvTCArgs> &go, void **plan_out);
+int gru_chain_launch(void *plan, cudaStream_t st);
+void gru_chain_destroy(void *plan);
+// tensor-map builders (shared with dcn_fused.cu, wgrad_tc.cu)
 int tc_make_amap(const SplitTensor &t, int box_w, int box_h, CUtensorMap *out);
 int tc_make_bmap(const void *w, int npad, int nkb, int box_rows, CUtensorMap *out);
-// tc_conv_halo.cu: persistent halo-reuse kernel for multi-wave 3x3 layers (kernel_ver 4)
-bool conv_tc_halo_plan(int npad, int staging_bufs, int *a_stages, int *b_stages);
-int tc_make_omap(const SplitTensor &t, int box_w, int box_h, CUtensorMap *out);
-int tc_make_omap_f32(float *base, int n_img, int H, int W, int C, int box_w, int box_h, CUtensorMap *out);
-int conv_tc_halo_launch(const ConvTCArgs &args, cudaStream_t st);
-// tc_conv3.cu
-bool conv_tc3_plan(int npad, int *a_stages, int *b_stages);
-int conv_tc3_launch(const ConvTCArgs &args, cudaStream_t st);
 
 // w: fp32 [cout, cin, k, k] (device) -> packed split bf16 [2][nkb][npad][64]; kb = chunk*ntaps + tap
 int pack_conv_weight(const float *w, int cout, int cin, int ksz, void *dst, cudaStream_t st);

@@ -10,7 +10,7 @@
 //   esr_mse_loss         mean((p - t)^2) and its gradient
 //   esr_adam_step        torch.optim.Adam semantics (L2 weight decay folded into the gradient, optional amsgrad)
 //
-// Stride-1 layers with 64-multiple input channels run on the tcgen05 implicit-GEMM kernel of tc_conv.cu (fp32 -> split
+// Stride-1 layers with 64-multiple input channels run on the wgmma implicit-GEMM kernel of tc_conv.cu (fp32 -> split
 // bf16, 3-pass product, fp32 accumulate): the forward directly, dx as the same kernel over g with the weights transposed
 // and rotated, and dw as a tensor-core reduction over pixels (k_wgrad_tc below, MN-major operands).  Every other shape
 // (the <= 32-channel full-resolution layers, stride-2 encoder convs, 1- and 2-channel heads) uses the CUDA-core kernels

@@ -1,27 +1,28 @@
-// wgrad_tc.cu -- weight gradient of a stride-1 3x3 (pad 1) / 1x1 convolution on the tensor cores.
+// wgrad_tc.cu -- weight gradient of a stride-1 3x3 (pad 1) / 1x1 convolution on the tensor cores (sm_90a, wgmma).
 //
 //   dw[co, ci, ky, kx] = sum over (image, y, x) of g[image, y, x, co] * x[image, y + ky - 1, x + kx - 1, ci]
 //
 // is, per tap, a GEMM whose reduction dimension is the PIXEL index: D[a-channel, b-channel] += A^T B with A and B both
 // stored pixel-major (NHWC rows of 64 channels = one 128-byte shared-memory row per pixel).  That is exactly the
-// MN-major SWIZZLE_128B operand layout of tcgen05 (canonical ((8,n),(8,k)) : ((1,LBO),(8,SBO)) in 16-byte units: 64
-// channels contiguous in a row, 8 pixel rows per 1024-byte swizzle atom, SBO = 1024 between K atoms, LBO = distance
-// between 64-channel tiles), so the same TMA boxes the forward kernel loads (64 ch x TW x TH pixels, tap shift + zero
-// fill = padding) feed the MMA directly -- no transposition anywhere.  fp32 parity: operands are split bf16 (hi, lo),
-// three MMAs per K step (lo*hi + hi*lo + hi*hi) into fp32 TMEM accumulators, like the forward.
+// MN-major SWIZZLE_128B operand layout of wgmma (canonical ((8,n),(8,k)) : ((1,LBO),(8,SBO)) in 16-byte units: 64
+// channels contiguous in a row, 8 pixel rows per 1024-byte swizzle atom, SBO = 1024 between K atoms), so the same TMA
+// boxes the forward kernel loads (64 ch x TW x TH pixels, tap shift + zero fill = padding) feed the MMA directly -- no
+// transposition anywhere.  fp32 parity: operands are split bf16 (hi, lo), three MMAs per K step (lo*hi + hi*lo + hi*hi)
+// into fp32 accumulators, like the forward.
 //
-// One CTA owns (128 M-side channels, 64 N-side channels, a group of <= 5 taps, a slice of the pixel tiles): it keeps one
-// 128 x 64 fp32 accumulator per tap in TMEM (5 x 64 = 320 of the 512 columns; all 9 taps would need 576), streams its
-// pixel tiles through a TMA/mbarrier pipeline (the unshifted tensor once per tile, the shifted one once per tap) and adds
+// One CTA owns (128 M-side channels, 64 N-side channels, a group of <= 3 taps, a slice of the pixel tiles): each of its two
+// consumer warpgroups keeps one 64 x 64 fp32 accumulator per tap in registers (M-side channels [64 w, 64 w + 64)), streams
+// the pixel tiles through a TMA/mbarrier pipeline (the unshifted tensor once per tile, the shifted one once per tap) and adds
 // its partial sums to dw with fp32 atomics at the end.  Which tensor sits on the 128-row M side is chosen per layer:
 // g (Cout >= 128) or x (Cout == 64 and Cin >= 128); a 64-channel tensor on the M side is loaded twice (rows 64..127
-// ignored).  Warps: 0 = TMA producer, 1 = MMA issuer + TMEM owner, 2..5 = epilogue.
+// ignored).  Warps: 0-7 = MMA + epilogue (two warpgroups), 8 = TMA producer.
 #include "tc_common.cuh"
 #include "net.cuh"
 
 namespace esr {
 
-constexpr int WG_THREADS = 192;
+constexpr int WG_THREADS = 288;
+constexpr int WG_TAPS = 3;                            // taps per CTA (accumulators: 3 x 32 registers per thread)
 constexpr uint32_t WG_TILE = TC_BLOCK_M * 128u;       // one 64-channel x 128-pixel plane: 16 KB
 
 struct WgradArgs {
@@ -29,29 +30,9 @@ struct WgradArgs {
     float *dw;                        // [Cout][Cin][KK]
     int Cout, CoutPad, Cin, KK;       // g has CoutPad (64-multiple) channels, the first Cout are real
     int a_is_x;                       // 1: M side = x channels (shifted per tap), N side = g; 0: M side = g, N side = x
-    CUtensorMap hmap;                 // halo mode: x as (64 ch, TW + 2, TH + 2, 1, 1) boxes
-    int halo;                         // 1: ONE halo tile of x per pixel tile feeds all taps (shifted MN-major descriptors)
     int m_blocks, n_chunks, groups;   // grid decomposition
     int n_img, H, W, TW, TH, tiles_x, tiles_y, slices;
 };
-
-// MN-major, 128B-swizzled operand: start | LBO (between 64-channel tiles) | SBO = 1024 (between 8-pixel K atoms)
-__device__ __forceinline__ uint64_t umma_desc_mn(uint32_t smem_addr, uint32_t lbo_bytes)
-{
-    uint64_t d = 0;
-    d |= (uint64_t)((smem_addr & 0x3FFFFu) >> 4);
-    d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFFu) << 16;
-    d |= (uint64_t)(1024 >> 4) << 32;
-    d |= (uint64_t)1 << 46;
-    d |= (uint64_t)2 << 61;
-    return d;
-}
-
-// lower word of the same descriptor (the upper word is UMMA_HI_1024); advancing the operand by n bytes is lo + n / 16
-__device__ __forceinline__ uint32_t umma_desc_mn_lo(uint32_t smem_addr, uint32_t lbo_bytes)
-{
-    return ((smem_addr & 0x3FFFFu) >> 4) | (((lbo_bytes >> 4) & 0x3FFFu) << 16);
-}
 
 __global__ void __launch_bounds__(WG_THREADS, 1) k_wgrad_tc(const __grid_constant__ WgradArgs a)
 {
@@ -60,12 +41,10 @@ __global__ void __launch_bounds__(WG_THREADS, 1) k_wgrad_tc(const __grid_constan
     // shared memory: [once buffers x2][per-tap ring x2][barriers]; sizes depend on which tensor is on the M side
     const uint32_t m_bytes = 4u * WG_TILE, n_bytes = 2u * WG_TILE;      // M side: 2 tiles x 2 planes; N side: 1 tile x 2 planes
     const uint32_t once_bytes = a.a_is_x ? n_bytes : m_bytes;           // the unshifted tensor (g)
-    const uint32_t halo_plane = ((uint32_t)((a.TW + 2) * (a.TH + 2)) * 128u + 1023u) & ~1023u;
-    const uint32_t tap_bytes = a.halo ? 2u * halo_plane : (a.a_is_x ? m_bytes : n_bytes);   // the shifted tensor (x), or its halo box
+    const uint32_t tap_bytes = a.a_is_x ? m_bytes : n_bytes;            // the shifted tensor (x)
     const uint32_t once_base = smem_base, ring_base = smem_base + 2u * once_bytes;
     const uint32_t bar_base = ring_base + 2u * tap_bytes;
     const uint32_t bar_gfull = bar_base, bar_gempty = bar_base + 16u, bar_xfull = bar_base + 32u, bar_xempty = bar_base + 48u;
-    const uint32_t bar_accum = bar_base + 64u, tmem_slot = bar_base + 72u;
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
 
     // block -> (M block, N chunk, tap group, slice)
@@ -73,9 +52,9 @@ __global__ void __launch_bounds__(WG_THREADS, 1) k_wgrad_tc(const __grid_constan
     const int slice = bid % a.slices; bid /= a.slices;
     const int grp = bid % a.groups; bid /= a.groups;
     const int nch = bid % a.n_chunks; const int mblk = bid / a.n_chunks;
-    const int tap0 = grp == 0 ? 0 : 5;
-    const int ntap = a.KK == 1 ? 1 : (grp == 0 ? 5 : 4);
- const int m_ch = a.a_is_x ? a.Cin : a.CoutPad;               // channels of the M-side tensor as stored
+    const int tap0 = grp * WG_TAPS;
+    const int ntap = a.KK == 1 ? 1 : WG_TAPS;
+    const int m_ch = a.a_is_x ? a.Cin : a.CoutPad;               // channels of the M-side tensor as stored
     const int m_real = a.a_is_x ? a.Cin : a.Cout;
     const int m0 = mblk * 128;
     const bool m_dup = m0 + 64 >= m_ch;                                  // only 64 channels left on the M side
@@ -84,20 +63,14 @@ __global__ void __launch_bounds__(WG_THREADS, 1) k_wgrad_tc(const __grid_constan
 
     if (threadIdx.x == 0) {
         for (int s = 0; s < 2; ++s) {
-            mbar_init(bar_gfull + 8u * s, 1); mbar_init(bar_gempty + 8u * s, 1);
-            mbar_init(bar_xfull + 8u * s, 1); mbar_init(bar_xempty + 8u * s, 1);
+            mbar_init(bar_gfull + 8u * s, 1); mbar_init(bar_gempty + 8u * s, 8);
+            mbar_init(bar_xfull + 8u * s, 1); mbar_init(bar_xempty + 8u * s, 8);
         }
-        mbar_init(bar_accum, 1);
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
-    if (warp == 1) tmem_alloc(tmem_slot, 512);
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    uint32_t tmem_base;
-    asm volatile("ld.shared.b32 %0, [%1];" : "=r"(tmem_base) : "r"(tmem_slot));
 
-    if (warp == 0) {
+    if (warp == 8) {
         if (elect_one_sync()) {
             uint32_t gs = 0, gph = 0, xs = 0, xph = 0;
             for (int t = slice; t < n_tiles; t += a.slices) {
@@ -118,16 +91,6 @@ __global__ void __launch_bounds__(WG_THREADS, 1) k_wgrad_tc(const __grid_constan
                     tma_load_5d(&a.gmap, bar_gfull + 8u * gs, gb + WG_TILE, n0, x0, y0, img, 1);
                 }
                 if (++gs == 2) { gs = 0; gph ^= 1u; }
-                if (a.halo) {
-                    // ---- ONE halo box of x for all taps of this pixel tile (hi and lo planes); zero fill outside = padding
-                    mbar_wait(bar_xempty + 8u * xs, xph ^ 1u);
-                    mbar_expect_tx(bar_xfull + 8u * xs, 2u * (uint32_t)((a.TW + 2) * (a.TH + 2)) * 128u);
-                    const uint32_t xb = ring_base + xs * tap_bytes;
-                    tma_load_5d(&a.hmap, bar_xfull + 8u * xs, xb, n0, x0 - 1, y0 - 1, img, 0);
-                    tma_load_5d(&a.hmap, bar_xfull + 8u * xs, xb + halo_plane, n0, x0 - 1, y0 - 1, img, 1);
-                    if (++xs == 2) { xs = 0; xph ^= 1u; }
-                    continue;
-                }
                 // ---- x tile(s), one per tap, shifted; out-of-image pixels are zero-filled = the conv padding
                 for (int j = 0; j < ntap; ++j) {
                     const int tap = tap0 + j;
@@ -149,93 +112,63 @@ __global__ void __launch_bounds__(WG_THREADS, 1) k_wgrad_tc(const __grid_constan
                 }
             }
         }
-    } else if (warp == 1) {
-        if (elect_one_sync()) {
-            // MN-major A and B (bits 15, 16), fp32 accumulate, bf16 operands, M = 128, N = 64
-            const uint32_t idesc = umma_idesc(TC_BLOCK_M, 64) | (1u << 15) | (1u << 16);
-            uint32_t gs = 0, gph = 0, xs = 0, xph = 0;
-            bool first = true;
-            for (int t = slice; t < n_tiles; t += a.slices) {
-                mbar_wait(bar_gfull + 8u * gs, gph);
-                const uint32_t gb = once_base + gs * once_bytes;
-                if (a.halo) {
-                    mbar_wait(bar_xfull + 8u * xs, xph);
-                    tc_fence_after();
-                    const uint32_t xb = ring_base + xs * tap_bytes;
-                    const uint32_t m_hi = gb, m_lo = gb + 2u * WG_TILE;
-                    const uint32_t hw = (uint32_t)(a.TW + 2);
-                    for (int j = 0; j < ntap; ++j) {
-                        const int tap = tap0 + j, ky = tap / 3, kx = tap % 3;
-                        const uint32_t d = tmem_base + (uint32_t)j * 64u;
-#pragma unroll
-                        for (int k = 0; k < 8; ++k) {                    // K step k = tile row k: 16 pixels = 16 rows of the halo box
-                            const uint32_t sh = (((uint32_t)(k + ky)) * hw + (uint32_t)kx) * 128u;
-                            const uint64_t dah = umma_desc(umma_desc_mn_lo(m_hi, WG_TILE) + 128u * k, UMMA_HI_1024), dal = umma_desc(umma_desc_mn_lo(m_lo, WG_TILE) + 128u * k, UMMA_HI_1024);
-                            const uint64_t dbh = umma_desc(umma_desc_mn_lo(xb, WG_TILE) + (sh >> 4), UMMA_HI_1024), dbl = umma_desc(umma_desc_mn_lo(xb + halo_plane, WG_TILE) + (sh >> 4), UMMA_HI_1024);
-                            umma_bf16(d, dal, dbh, idesc, (first && k == 0) ? 0u : 1u);
-                            umma_bf16(d, dah, dbl, idesc, 1u);
-                            umma_bf16(d, dah, dbh, idesc, 1u);
-                        }
-                    }
-                    umma_commit(bar_xempty + 8u * xs);
-                    if (++xs == 2) { xs = 0; xph ^= 1u; }
-                    umma_commit(bar_gempty + 8u * gs);
-                    if (++gs == 2) { gs = 0; gph ^= 1u; }
-                    first = false;
-                    continue;
-                }
-                for (int j = 0; j < ntap; ++j) {
-                    mbar_wait(bar_xfull + 8u * xs, xph);
-                    tc_fence_after();
-                    const uint32_t xb = ring_base + xs * tap_bytes;
-                    const uint32_t m_hi = a.a_is_x ? xb : gb, m_lo = m_hi + 2u * WG_TILE;       // M side planes (2 tiles each)
-                    const uint32_t n_hi = a.a_is_x ? gb : xb, n_lo = n_hi + WG_TILE;            // N side planes
-                    const uint32_t d = tmem_base + (uint32_t)j * 64u;
-#pragma unroll
-                    for (int k = 0; k < 8; ++k) {                        // 8 x (K = 16 pixels = 16 rows = 2048 bytes)
-                        const uint64_t dah = umma_desc(umma_desc_mn_lo(m_hi, WG_TILE) + 128u * k, UMMA_HI_1024), dal = umma_desc(umma_desc_mn_lo(m_lo, WG_TILE) + 128u * k, UMMA_HI_1024);
-                        const uint64_t dbh = umma_desc(umma_desc_mn_lo(n_hi, WG_TILE) + 128u * k, UMMA_HI_1024), dbl = umma_desc(umma_desc_mn_lo(n_lo, WG_TILE) + 128u * k, UMMA_HI_1024);
-                        umma_bf16(d, dal, dbh, idesc, (first && k == 0) ? 0u : 1u);
-                        umma_bf16(d, dah, dbl, idesc, 1u);
-                        umma_bf16(d, dah, dbh, idesc, 1u);
-                    }
-                    umma_commit(bar_xempty + 8u * xs);
-                    if (++xs == 2) { xs = 0; xph ^= 1u; }
-                }
-                umma_commit(bar_gempty + 8u * gs);
-                if (++gs == 2) { gs = 0; gph ^= 1u; }
-                first = false;
-            }
-            umma_commit(bar_accum);
-        }
-    } else if (slice < n_tiles) {
-        // ===================== epilogue: TMEM -> fp32 atomics into dw =====================
-        const int quad = warp & 3;
-        const int m = quad * 32 + lane;                                  // accumulator row = M-side channel
-        const bool row_ok = (m < 64 || !m_dup) && (m0 + m < m_real);
-        mbar_wait_backoff(bar_accum, 0);
-        tc_fence_after();
-        for (int j = 0; j < ntap; ++j) {
-            const int tap = tap0 + j;
-#pragma unroll 1
-            for (int half = 0; half < 2; ++half) {
-                uint32_t raw[32];
-                tmem_ld32(tmem_base + ((uint32_t)(quad * 32) << 16) + (uint32_t)(j * 64 + half * 32), raw);
-                if (row_ok) {
-#pragma unroll
-                    for (int c = 0; c < 32; ++c) {
-                        const int nc = n0 + half * 32 + c;
-                        const int co = a.a_is_x ? nc : m0 + m, ci = a.a_is_x ? m0 + m : nc;
-                        if (co < a.Cout) atomicAdd(a.dw + ((size_t)co * a.Cin + ci) * a.KK + tap, __uint_as_float(raw[c]));
-                    }
-                }
-            }
-        }
+        return;
     }
 
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 1) { tc_fence_after(); tmem_dealloc(tmem_base, 512); }
+    // ===================== consumers: warpgroup wg = M-side channels [m0 + 64 wg, +64) =====================
+    const int wg = warp >> 2;
+    float acc[WG_TAPS][32];
+#pragma unroll
+    for (int j = 0; j < WG_TAPS; ++j)
+#pragma unroll
+        for (int i = 0; i < 32; ++i) acc[j][i] = 0.0f;
+    uint32_t gs = 0, gph = 0, xs = 0, xph = 0;
+    for (int t = slice; t < n_tiles; t += a.slices) {
+        mbar_wait(bar_gfull + 8u * gs, gph);
+        const uint32_t gb = once_base + gs * once_bytes;
+#pragma unroll
+        for (int j = 0; j < WG_TAPS; ++j) {
+            if (j >= ntap) break;
+            mbar_wait(bar_xfull + 8u * xs, xph);
+            const uint32_t xb = ring_base + xs * tap_bytes;
+            const uint32_t m_hi = (a.a_is_x ? xb : gb) + (uint32_t)wg * WG_TILE, m_lo = m_hi + 2u * WG_TILE;   // this warpgroup's M tile
+            const uint32_t n_hi = a.a_is_x ? gb : xb, n_lo = n_hi + WG_TILE;                                   // N side planes
+            const uint64_t dah = wgmma_desc(m_hi, WG_TILE), dal = wgmma_desc(m_lo, WG_TILE);
+            const uint64_t dbh = wgmma_desc(n_hi, WG_TILE), dbl = wgmma_desc(n_lo, WG_TILE);
+            acc_fence<32>(acc[j]);
+            wgmma_fence();
+#pragma unroll
+            for (int k = 0; k < 8; ++k) {                        // 8 x (K = 16 pixels = 16 rows = 2048 bytes)
+                wgmma_rows<64, 1>(acc[j], dal + 128 * k, dbh + 128 * k);
+                wgmma_rows<64, 1>(acc[j], dah + 128 * k, dbl + 128 * k);
+                wgmma_rows<64, 1>(acc[j], dah + 128 * k, dbh + 128 * k);
+            }
+            wgmma_commit();
+            wgmma_wait<0>();
+            acc_fence<32>(acc[j]);
+            if (lane == 0) mbar_arrive(bar_xempty + 8u * xs);
+            if (++xs == 2) { xs = 0; xph ^= 1u; }
+        }
+        if (lane == 0) mbar_arrive(bar_gempty + 8u * gs);
+        if (++gs == 2) { gs = 0; gph ^= 1u; }
+    }
+    if (slice >= n_tiles) return;
+
+    // ===================== epilogue: accumulator fragments -> fp32 atomics into dw =====================
+    const int w = warp & 3;
+#pragma unroll
+    for (int j = 0; j < WG_TAPS; ++j) {
+        if (j >= ntap) break;
+        const int tap = tap0 + j;
+#pragma unroll
+        for (int i = 0; i < 32; ++i) {
+            const int m = wg * 64 + 16 * w + (lane >> 2) + 8 * ((i >> 1) & 1);   // accumulator row = M-side channel
+            const int nc = n0 + 8 * (i >> 2) + 2 * (lane & 3) + (i & 1);        // column = N-side channel
+            const bool row_ok = (m < 64 || !m_dup) && (m0 + m < m_real);
+            const int co = a.a_is_x ? nc : m0 + m, ci = a.a_is_x ? m0 + m : nc;
+            if (row_ok && co < a.Cout) atomicAdd(a.dw + ((size_t)co * a.Cin + ci) * a.KK + tap, acc[j][i]);
+        }
+    }
 }
 
 // x_split: split NHWC [2][B][H][W][Cin]; g_split: split NHWC [2][B][H][W][CoutPad] (channels >= Cout zero); dw pre-zeroed.
@@ -250,27 +183,23 @@ int wgrad_tc(const __nv_bfloat16 *x_split, const __nv_bfloat16 *g_split, int B, 
     memset(&a, 0, sizeof(a));
     a.dw = dw; a.Cout = Cout; a.Cin = Cin; a.KK = ksz * ksz;
     a.a_is_x = (Cout == 64 && Cin >= 128) ? 1 : 0;
-    // halo mode: 16 x 8 tiles (a K step = one 16-pixel tile row, contiguous in the halo box); ESR_WGRAD_NO_HALO=1 turns it off
-    a.halo = (ksz == 3 && !a.a_is_x && W >= 12 && getenv("ESR_WGRAD_NO_HALO") == nullptr) ? 1 : 0;
-    a.TW = a.halo ? 16 : (W >= 24 ? 32 : (W >= 12 ? 16 : 8)); a.TH = TC_BLOCK_M / a.TW;
+    a.TW = W >= 24 ? 32 : (W >= 12 ? 16 : 8); a.TH = TC_BLOCK_M / a.TW;
     if ((rc = tc_make_amap(gs, a.TW, a.TH, &a.gmap))) return rc;
     if ((rc = tc_make_amap(xs, a.TW, a.TH, &a.xmap))) return rc;
-    if (a.halo && (rc = tc_make_amap(xs, a.TW + 2, a.TH + 2, &a.hmap))) return rc;
     const int m_ch = a.a_is_x ? Cin : CoutPad, n_ch = a.a_is_x ? CoutPad : Cin;
     a.CoutPad = CoutPad;
-    a.m_blocks = (m_ch + 127) / 128; a.n_chunks = n_ch / 64; a.groups = ksz == 3 ? 2 : 1;
+    a.m_blocks = (m_ch + 127) / 128; a.n_chunks = n_ch / 64; a.groups = ksz == 3 ? 9 / WG_TAPS : 1;
     a.n_img = B; a.H = H; a.W = W;
     a.tiles_x = (W + a.TW - 1) / a.TW; a.tiles_y = (H + a.TH - 1) / a.TH;
     const int n_tiles = B * a.tiles_x * a.tiles_y, base = a.m_blocks * a.n_chunks * a.groups;
     // one CTA per SM.  (Every CTA ends with 128 x 64 x taps fp32 atomics; giving small problems fewer, longer CTAs was measured
-    // slower on B200: min 6 tiles per CTA +0.3 ms, min 16 +2 ms per cfg2 training iteration -- ESR_WGRAD_MIN_TILES to retest.)
+    // slower: min 6 tiles per CTA +0.3 ms, min 16 +2 ms per cfg2 training iteration -- ESR_WGRAD_MIN_TILES to retest.)
     int slices = (dev_info().sm_count + base - 1) / base;
     static const int min_tiles = getenv("ESR_WGRAD_MIN_TILES") ? atoi(getenv("ESR_WGRAD_MIN_TILES")) : 1;
     if (slices > n_tiles / min_tiles) slices = n_tiles / min_tiles;
     if (slices < 1) slices = 1;
     a.slices = slices;
-    const size_t halo_plane = align_up((size_t)(a.TW + 2) * (a.TH + 2) * 128, 1024);
-    const size_t smem = 1024 + 2 * (size_t)(4 * WG_TILE) + 2 * (a.halo ? 2 * halo_plane : (size_t)(2 * WG_TILE)) + 128;
+    const size_t smem = 1024 + 2 * (size_t)(4 * WG_TILE) + 2 * (size_t)(2 * WG_TILE) + 64;
     static size_t attr_done = 0;
     if (smem > attr_done) {
         ESR_CUDA_CHECK(cudaFuncSetAttribute(k_wgrad_tc, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));

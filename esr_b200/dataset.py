@@ -1,6 +1,6 @@
 """Host-side mirrors of the dataset glue on the hot path (no HDF5 I/O here: h5py is absent and no data ships; the
 reader itself is SURVEY.md 8f "next").  Same names, argument meaning and results as the reference methods, but the
-tensors live on the GPU and the encodings are the sm_100a kernels of esr_b200.encodings.
+tensors live on the GPU and the encodings are the sm_90a kernels of esr_b200.encodings.
 
   event_formatting(events)                                   dataloader/base_dataset.py:26-33
   create_normalized_events(events, sensor_resolution)        dataloader/h5dataset.py:508-518

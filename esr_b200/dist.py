@@ -1,4 +1,4 @@
-"""Multi-GPU plumbing: one process per GPU, torch.distributed (NCCL on the B200 box, gloo in CPU tests).
+"""Multi-GPU plumbing: one process per GPU, torch.distributed (NCCL on the GPUs, gloo in CPU tests).
 
 The hot path shards by batch (independent sequences, no BatchNorm; SURVEY.md 8e): inference, encoding and
 redistribution need NO collective; ranks only meet to agree on timings.  Training adds exactly one exchange --

@@ -1,4 +1,4 @@
-"""Make the reference's own scripts pick up the B200 implementation without editing them.
+"""Make the reference's own scripts pick up the H100 implementation without editing them.
 
     import esr_b200.dropin; esr_b200.dropin.install()        # before `from models.model import *`
 

@@ -9,7 +9,7 @@ Same names, positional arguments and side effects as the reference:
   cython_event_redistribute(event_stack, mode)    encodings.py:466-484
   multiprocess_cython(event_stack, mode)          encodings.py:495-533 (per-sample calls, no process pool)
   stack2cnt(stack)                                encodings.py:652-670
-plus the batched entry point the B200 pipeline uses:
+plus the batched entry point the GPU pipeline uses:
   encode_frames(xs, ys, ps, frame_off, lr_size, hr_size)  -> [F,2,kH,kW] on the GPU, fusing the LR->HR lift of
                                                             dataloader/h5dataset.py:508-528.
 CPU tensors are accepted (copied to the current CUDA device, result and in-place side effects copied back);

@@ -1,5 +1,5 @@
 """Drop-in for the reference's `dataloader.cython_event_redistribute.event_redistribute` Cython module
-(event_redistribute.pyx:17-153), backed by the sm_100a kernels.  numpy in, numpy out, like the original."""
+(event_redistribute.pyx:17-153), backed by the sm_90a kernels.  numpy in, numpy out, like the original."""
 import numpy as np
 import torch
 

@@ -4,7 +4,7 @@ The reference reads HDF5 event files through h5py, one Python `__getitem__` per 
 (dataloader/h5dataset.py:32-38, 147-161, 196-270, 451-506; file layout written by
 generate_dataset/tools/event_packagers.py:121-224: groups `{ori,down2,down4,down8,down16}_events/{xs:int16, ys:int16,
 ts:float64, ps:float64}`, `ori_images/image%09d` with a `timestamp` attribute, file attribute `sensor_resolution`).
-At B200 speed (20 k LR frames/s) that loader is the limiter.  Here:
+At the GPU pipeline's speed that loader is the limiter.  Here:
 
   * `EventStore`  -- the same columns in ONE flat file (4 KiB header with a JSON table, 4 KiB-aligned raw little-endian arrays),
     opened with numpy.memmap and (optionally) copied once into pinned host memory or HBM.  `convert_hdf5` makes one from a

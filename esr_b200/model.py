@@ -1,4 +1,4 @@
-"""B200 implementation of the reference's `models/model.py` network class.
+"""H100 implementation of the reference's `models/model.py` network class.
 
 `DeepRecurrNet` keeps the reference's constructor signature, `forward(BxNx2xHxW) -> Bx2xHxW`, `reset_states()` and
 state_dict key names (models/model.py:294-344; 68 tensors, SURVEY 8b), so a reference checkpoint loads with
@@ -6,7 +6,7 @@ state_dict key names (models/model.py:294-344; 68 tensors, SURVEY 8b), so a refe
 The parameters are ordinary `nn.Parameter`s (DDP-wrappable); the forward pass is the C++/CUDA plan behind
 `esr_net_*` (include/esr_b200.h).  There is no PyTorch/CPU fallback: a CPU tensor or a missing library raises.
 
-Two execution paths, both sm_100a kernels behind the C ABI:
+Two execution paths, both sm_90a kernels behind the C ABI:
   * torch.no_grad(): the fused inference plan (esr_net_*), states kept inside the plan's workspace;
   * gradients enabled (training, train_ours_cnt_seq.py:217-232): esr_b200.train.forward_window -- the same network
     composed from differentiable operators (esr_conv2d_forward/backward, esr_dcn_v2_forward/backward), with the
@@ -155,7 +155,7 @@ class DeepRecurrNet(nn.Module):
         ok = (c["inch"] == 2 and c["basech"] == 8 and c["num_frame"] == 3 and c["norm"] is None and c["activation"] == "relu"
               and c["has_ltc"] and c["has_gtc"] and not c["gtc_frozen"] and c["has_dcnatten"] and c["has_scaleaggre"])
         if not ok:
-            raise _lib.ESRError("esr_b200.DeepRecurrNet: the sm_100a plan implements the shipped configuration "
+            raise _lib.ESRError("esr_b200.DeepRecurrNet: the sm_90a plan implements the shipped configuration "
                                 "(inch=2, basech=8, num_frame=3, norm=None, relu, all blocks on; "
                                 f"config/train_ours_enfssyn.yml:21-26); got {c}")
 

@@ -5,7 +5,7 @@ through time across windows), calls backward once, lets DDP all-reduce the 1 813
 Adam(lr, weight_decay, amsgrad).  Here
 
   * every ConvLayer (models/submodules.py:159-200) is `conv2d` below: an autograd.Function whose forward AND backward
-    are the sm_100a operators esr_conv2d_forward / esr_conv2d_backward (tcgen05 implicit GEMM for the 64-multiple
+    are the sm_90a operators esr_conv2d_forward / esr_conv2d_backward (wgmma implicit GEMM for the 64-multiple
     layers incl. dx and dw, CUDA-core kernels for the narrow full-resolution layers; include/esr_b200.h);
   * DCN_sep (models/DCNv2/dcn_v2.py:17-68) is `dcn_v2`: esr_dcn_v2_forward / esr_dcn_v2_backward;
   * the loss and the optimizer are esr_mse_loss / esr_adam_step (one launch over the flat parameter buffer);

@@ -1,5 +1,5 @@
 /*
- * esr_b200.h -- C ABI of libesr_b200.so, the B200 (sm_100a) implementation of WarranWeng/ESR's
+ * esr_b200.h -- C ABI of libesr_b200.so, the H100 (sm_90a) implementation of WarranWeng/ESR's
  * per-timestep hot path.  Plain pointers and sizes only; every pointer is a DEVICE pointer unless
  * its name ends in _host.  The caller owns every buffer and the stream; the library allocates no
  * user-visible memory (workspaces are sized by *_workspace_bytes and passed in).  All functions return
@@ -22,7 +22,7 @@ extern "C" {
 #define ESR_EINVAL (-1)       /* bad argument */
 #define ESR_ENEGCOUNT (-2)    /* negative rounded count: the reference raises ValueError (cnt2event.pyx:71) */
 #define ESR_ECUDA (-3)        /* CUDA runtime / driver error */
-#define ESR_EUNSUPPORTED (-4) /* configuration outside what the sm_100a kernels implement */
+#define ESR_EUNSUPPORTED (-4) /* configuration outside what the sm_90a kernels implement */
 #define ESR_EWORKSPACE (-5)   /* workspace too small */
 
 typedef void *esr_stream_t; /* cudaStream_t */
@@ -117,7 +117,7 @@ int esr_cnt2event_fused(const float *vals, int B, int H, int W, const void *tabl
                         esr_stream_t stream);
 
 /* ---------------------------------------------------------------------------------------------
- * Tensor-core convolution (tcgen05, TMA-tiled implicit GEMM), layer-level entry point.
+ * Tensor-core convolution (wgmma, TMA-tiled implicit GEMM), layer-level entry point.
  * Replaces: every stride-1 nn.Conv2d at feature resolution in models/model.py / models/submodules.py
  * (3x3 pad 1 or 1x1; Cin a multiple of 64, Cout <= 256), including torch.cat inputs (K-split over up to 3
  * sources), the fused bias / residual / activation tail of ConvLayer / ResidualBlock
@@ -211,7 +211,7 @@ int esr_net_set_states(esr_net_t net, const float *states, esr_stream_t stream);
  * --------------------------------------------------------------------------------------------- */
 size_t esr_dcn_v2_workspace_bytes(int B, int H, int W);   /* the configuration ESR uses (64 -> 64, 3x3, s1 p1 d1, 8 groups) */
 /* workspace for ANY configuration the reference operator accepts (backward = 1: for esr_dcn_v2_backward).  The configuration
- * of models/model.py:173 runs on the tcgen05 path; every other one (the reference's own tests use 2 -> 2 channels and
+ * of models/model.py:173 runs on the wgmma path; every other one (the reference's own tests use 2 -> 2 channels and
  * deformable_groups 1 / 2, models/DCNv2/testcuda.py:14-17,169-180) on fp32 CUDA-core kernels (csrc/dcn_generic.cu). */
 size_t esr_dcn_v2_workspace_bytes_ex(int B, int C, int H, int W, int Co, int kernel, int stride, int pad, int dilation,
                                      int deformable_group, int backward);

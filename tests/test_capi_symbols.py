@@ -1,4 +1,4 @@
-"""CPU: libesr_b200.so builds for sm_100a, loads, and exports every symbol include/esr_b200.h declares."""
+"""CPU: libesr_b200.so builds for sm_90a, loads, and exports every symbol include/esr_b200.h declares."""
 import ctypes
 import os
 import re

@@ -1,4 +1,4 @@
-"""GPU: the tcgen05 implicit-GEMM convolution (through the C ABI) against torch fp32 conv2d on the CPU.
+"""GPU: the wgmma implicit-GEMM convolution (through the C ABI) against torch fp32 conv2d on the CPU.
 Floating point => tolerance: 1e-4 relative to the output's max magnitude (the 3-pass split-bf16 product carries
 ~2^-17 relative operand error; the path-level budget from BASELINE.json is 1e-3)."""
 import pytest

@@ -109,7 +109,7 @@ def test_sequence_plan_equals_window_loop(dev, B, L, H, W):
 
 @pytest.mark.parametrize("B,L,H,W", [(1, 3, 16, 16), (2, 4, 36, 44), (1, 3, 72, 130)])
 def test_fused_dcn_equals_columns_path(dev, B, L, H, W, monkeypatch):
-    """The DCN kernel that samples straight into the swizzled tcgen05 operand tiles must give the same bits as the
+    """The DCN kernel that samples straight into the swizzled wgmma operand tiles must give the same bits as the
     two-kernel path (columns tensor in HBM + 1x1 GEMM): same sampling arithmetic, same MMA order."""
     sd = model_ref.seeded_state_dict(9)
     g = torch.Generator().manual_seed(L * 7 + H)
@@ -123,25 +123,42 @@ def test_fused_dcn_equals_columns_path(dev, B, L, H, W, monkeypatch):
     assert torch.equal(fused, cols), (fused - cols).abs().max().item()
 
 
+@pytest.mark.parametrize("B,L,H,W", [(1, 3, 16, 16), (2, 5, 36, 44), (1, 4, 72, 130)])
+def test_gru_chain_equals_per_step_launches(dev, B, L, H, W, monkeypatch):
+    """The ConvGRU recurrence as one cooperative kernel (persistent passes separated by grid barriers) must give the same bits as
+    two conv launches per step: same tiles, same MMA order, same epilogues; also for the carried states."""
+    sd = model_ref.seeded_state_dict(13)
+    g = torch.Generator().manual_seed(L * 11 + W)
+    frames = torch.poisson(torch.full((B, L, 2, H, W), 0.4), generator=g).to(dev)
+    n2 = _net(sd, dev)
+    with torch.no_grad():
+        steps = n2.forward_sequence(frames)
+        monkeypatch.setenv("ESR_GRU_CHAIN", "1")
+        n1 = _net(sd, dev)
+        chain = n1.forward_sequence(frames)
+    assert torch.equal(chain, steps), (chain - steps).abs().max().item()
+    for a, b in zip(n1.states(B, L, H, W), n2.states(B, L, H, W)):
+        assert torch.equal(a, b)
+
+
 @pytest.mark.parametrize("scale", [1.0, 60.0])
 def test_dcn_window_sampler_equals_gather_and_columns(dev, monkeypatch, scale):
-    """The L2-gather samplers (default) vs the opt-in TMA-staged sampling window vs the columns path: same bits, also when
-    the learned offsets are far larger than the window margin (scale 60 -> offsets of many pixels: every corner takes the
-    global-load fallback) and at ragged sizes."""
+    """The fused L2-gather sampler (default) vs the columns path: same bits, also when the learned offsets span many pixels
+    (scale 60) and at ragged sizes."""
     sd = model_ref.seeded_state_dict(12)
     sd["spacetime_fuse.dcn.conv_offset_mask.weight"] = sd["spacetime_fuse.dcn.conv_offset_mask.weight"] * scale
     sd["spacetime_fuse.dcn.conv_offset_mask.bias"] = sd["spacetime_fuse.dcn.conv_offset_mask.bias"] + (0.0 if scale == 1.0 else 2.5)
     g = torch.Generator().manual_seed(3)
     frames = torch.poisson(torch.full((2, 4, 2, 72, 104), 0.4), generator=g).to(dev)
     outs = []
-    for env in (None, "ESR_DCN_WINDOW", "ESR_DCN_COLUMNS"):
+    for env in (None, "ESR_DCN_COLUMNS"):
         if env:
             monkeypatch.setenv(env, "1")
         with torch.no_grad():
             outs.append(_net(sd, dev).forward_sequence(frames))
         if env:
             monkeypatch.delenv(env)
-    assert torch.equal(outs[0], outs[1]) and torch.equal(outs[0], outs[2])
+    assert torch.equal(outs[0], outs[1])
     ora = model_ref.OracleNet(sd)
     want = torch.cat([ora(frames[:, w:w + 3].cpu()) for w in range(2)], 0)
     assert _rel(outs[0].cpu(), want) <= REL

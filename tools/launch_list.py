@@ -31,5 +31,5 @@ print("| kernel | launches | total µs | share |\n|---|---|---|---|")
 for k, (n, t) in sorted(agg.items(), key=lambda kv: -kv[1][1]):
     print(f"| `{k}` | {n} | {t:.1f} | {100 * t / tot:.1f} % |")
 print(f"| **sum** | {len(step)} | {tot:.1f} | 100 % |")
-tc = sum(t for k, (n, t) in agg.items() if k.startswith(("k_conv_tc", "k_gru_chain", "k_dcn_fused")))
-print(f"\ntcgen05 kernels (k_conv_tc* + k_gru_chain_pipe + k_dcn_fused): {100 * tc / tot:.1f} % of the step under ncu.")
+tc = sum(t for k, (n, t) in agg.items() if k.startswith(("k_conv_tc", "k_dcn_fused")))
+print(f"\nwgmma kernels (k_conv_tc* + k_dcn_fused): {100 * tc / tot:.1f} % of the step.")

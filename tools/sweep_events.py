@@ -12,7 +12,7 @@ from esr_b200 import encodings as enc          # noqa: E402
 from esr_b200.expand import expand              # noqa: E402
 
 dev = torch.device("cuda:0")
-peak = 6574.1
+peak = 3350.0                                   # H100 SXM data sheet HBM3 GB/s; MEASURED_PEAKS.json overrides
 try:
     peak = json.load(open(os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "MEASURED_PEAKS.json")))["hbm_gbs"]
 except Exception:
