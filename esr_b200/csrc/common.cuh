@@ -20,6 +20,7 @@ inline void count_launch(int n = 1) { g_launches.fetch_add(n, std::memory_order_
         cudaError_t _e = (expr);                                                                   \
         if (_e != cudaSuccess) {                                                                   \
             esr::set_error("%s failed: %s (%s:%d)", #expr, cudaGetErrorString(_e), __FILE__, __LINE__); \
+            (void)cudaGetLastError();  /* a non-sticky error is reported once, not again by the next launch */ \
             return ESR_ECUDA;                                                                      \
         }                                                                                          \
     } while (0)

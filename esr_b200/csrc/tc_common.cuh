@@ -9,7 +9,9 @@ namespace esr {
 constexpr int TC_BLOCK_M = 128;                       // output pixels per tile: two warpgroups x 64 rows
 constexpr int TC_A_BYTES = TC_BLOCK_M * 128;          // one plane of one A tile: 128 rows x 64 bf16
 constexpr int TC_STG_LD = 68;                         // row stride (floats) of an epilogue staging tile: 64 columns + 4 (bank spread)
-constexpr uint32_t TC_STG_BYTES = 64u * TC_STG_LD * 4u; // one warpgroup's staging tile: 64 rows x 64 fp32 columns
+// one warpgroup's staging tile: 64 rows x 64 fp32 columns (the last row needs no bank padding: with it, npad = 256 at two
+// stages would exceed the 227 KB of shared memory an H100 block may use)
+constexpr uint32_t TC_STG_BYTES = (63u * TC_STG_LD + 64u) * 4u;
 
 // ------------------------------------------------------------------------------------------------
 // PTX wrappers
@@ -389,9 +391,13 @@ __device__ __forceinline__ void epilogue_chunk(const ConvTCArgs &a, const uint32
         float *op = a.out_f32 + pix * a.out_f32_C + n0;
         if ((a.out_f32_C & 3) == 0) {                 // 16-byte stores (conv_offset_mask: 216 channels)
 #pragma unroll
-            for (int q = 0; q < 8; ++q)
+            for (int q = 0; q < 8; ++q) {
                 if (n0 + 4 * q + 4 <= a.cout)
                     reinterpret_cast<float4 *>(op)[q] = make_float4(v[4 * q], v[4 * q + 1], v[4 * q + 2], v[4 * q + 3]);
+                else                                  // a cout that is not a multiple of 4 ends inside this quad
+                    for (int e = 0; e < 4; ++e)
+                        if (n0 + 4 * q + e < a.cout) op[4 * q + e] = v[4 * q + e];
+            }
         } else {
 #pragma unroll
             for (int j = 0; j < 32; ++j)

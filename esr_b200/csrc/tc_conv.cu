@@ -37,9 +37,12 @@ struct TcSmem {
 };
 struct TcRing { uint32_t s = 0, ph = 0; };
 
+// 1024: worst-case alignment of the ring; then the ring, the two staging tiles and the full / empty mbarriers.  npad = 256 at
+// the minimum of two stages takes exactly the 227 KB (232448 B) an H100 block may opt in to: nothing more fits beside it
+// (conv_tc_prepare refuses a width that does not fit instead of failing at launch).
 static size_t tc_smem_bytes(int npad, int stages)
 {
-    return 1024 + (size_t)stages * (2 * TC_A_BYTES + 2 * (size_t)npad * 128) + 2 * TC_STG_BYTES + 16 * (size_t)stages + 64;
+    return 1024 + (size_t)stages * (2 * TC_A_BYTES + 2 * (size_t)npad * 128) + 2 * TC_STG_BYTES + 16 * (size_t)stages;
 }
 __device__ __forceinline__ TcSmem tc_smem_layout(int np_max, int stages)
 {
@@ -298,6 +301,8 @@ int conv_tc_prepare(const ConvTCDesc &d, ConvTCArgs *args)
         if (2 * (tc_smem_bytes(a.npad, s2) + 1024) <= smem_cap) stages = s2;
     }
     if (stages > a.nkb) stages = a.nkb < 2 ? 2 : a.nkb;
+    ESR_REQUIRE(tc_smem_bytes(a.npad, stages) <= smem_cap, "conv_tc: npad=%d needs %zu B of shared memory, the device allows %zu",
+                a.npad, tc_smem_bytes(a.npad, stages), smem_cap);
     a.stages = stages;
     a.bias = d.bias;
     a.act = d.act; a.act_from = d.act_from; a.res_mode = d.res_mode; a.epi_mode = d.epi_mode;

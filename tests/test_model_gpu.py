@@ -107,20 +107,52 @@ def test_sequence_plan_equals_window_loop(dev, B, L, H, W):
             assert torch.equal(a, b)
 
 
-@pytest.mark.parametrize("B,L,H,W", [(1, 3, 16, 16), (2, 4, 36, 44), (1, 3, 72, 130)])
-def test_fused_dcn_equals_columns_path(dev, B, L, H, W, monkeypatch):
-    """The DCN kernel that samples straight into the swizzled wgmma operand tiles must give the same bits as the
-    two-kernel path (columns tensor in HBM + 1x1 GEMM): same sampling arithmetic, same MMA order."""
-    sd = model_ref.seeded_state_dict(9)
-    g = torch.Generator().manual_seed(L * 7 + H)
-    frames = torch.poisson(torch.full((B, L, 2, H, W), 0.4), generator=g).to(dev)
+def _fused_vs_columns_vs_oracle(dev, sd, frames, monkeypatch):
+    """forward_sequence with the fused DCN kernel == the columns path bit for bit, and within the bar of the oracle on the
+    first and last sequence of the batch (the sequences of a batch are independent)."""
+    import bench
+    B, L = frames.shape[:2]
     n1 = _net(sd, dev)
     with torch.no_grad():
-        fused = n1.forward_sequence(frames)
+        fused = n1.forward_sequence(frames.to(dev))
         monkeypatch.setenv("ESR_DCN_COLUMNS", "1")
         n2 = _net(sd, dev)
-        cols = n2.forward_sequence(frames)
+        cols = n2.forward_sequence(frames.to(dev))
     assert torch.equal(fused, cols), (fused - cols).abs().max().item()
+    torch.set_num_threads(bench.usable_cores())
+    idx = sorted({0, B - 1})
+    ora = model_ref.OracleNet(sd)
+    got = fused.view(L - 2, B, *fused.shape[1:])[:, idx].cpu()
+    for w in range(L - 2):
+        want = ora(frames[idx, w:w + 3].contiguous())
+        assert _rel(got[w], want) < REL, (w, _rel(got[w], want))
+
+
+@pytest.mark.parametrize("B,L,H,W", [(1, 3, 16, 16), (2, 4, 36, 44), (1, 3, 72, 130), (8, 8, 256, 256)])
+def test_fused_dcn_equals_columns_path(dev, B, L, H, W, monkeypatch):
+    """The DCN kernel that samples straight into the swizzled wgmma operand tiles must give the same bits as the
+    two-kernel path (columns tensor in HBM + 1x1 GEMM): same sampling arithmetic, same MMA order.  (8, 8, 256, 256) is
+    the benchmark's cfg2 input: 96 DCN images of 32x32, several tiles per CTA."""
+    sd = model_ref.seeded_state_dict(9)
+    g = torch.Generator().manual_seed(L * 7 + H)
+    frames = torch.poisson(torch.full((B, L, 2, H, W), 0.4), generator=g)
+    _fused_vs_columns_vs_oracle(dev, sd, frames, monkeypatch)
+
+
+def test_fused_dcn_lattice_offsets_on_the_borders(dev, monkeypatch):
+    """conv_offset_mask with zero weights and a bias of lattice offsets (multiples of 1/8, exact in fp32): every pixel of a
+    (group, tap) samples at the same offset, so integer offsets put samples exactly on -1, 0, H-1 and H (W-1, W) at the
+    image edges, and the half / eighth offsets land just inside and outside them."""
+    sd = model_ref.seeded_state_dict(10)
+    g = torch.Generator().manual_seed(10)
+    lattice = torch.tensor([-3.0, -2.0, -1.5, -1.0, -0.875, -0.5, -0.125, 0.0, 0.125, 0.5, 1.0, 1.125, 1.5, 2.0, 3.0])
+    w = sd["spacetime_fuse.dcn.conv_offset_mask.weight"]
+    b = sd["spacetime_fuse.dcn.conv_offset_mask.bias"].clone()
+    b[:144] = lattice[torch.randint(0, len(lattice), (144,), generator=g)]
+    sd["spacetime_fuse.dcn.conv_offset_mask.weight"] = torch.zeros_like(w)
+    sd["spacetime_fuse.dcn.conv_offset_mask.bias"] = b
+    frames = torch.poisson(torch.full((2, 4, 2, 64, 96), 0.4), generator=g)
+    _fused_vs_columns_vs_oracle(dev, sd, frames, monkeypatch)
 
 
 @pytest.mark.parametrize("B,L,H,W", [(1, 3, 16, 16), (2, 5, 36, 44), (1, 4, 72, 130)])
