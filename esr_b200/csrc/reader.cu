@@ -9,7 +9,9 @@
 //       are bit-identical;
 //   H5Dataset.get_events / get_gt_events + BaseDataset.event_formatting   dataloader/h5dataset.py:492-506,
 //       dataloader/base_dataset.py:26-33: int16 x / y and float64 t / p slices -> float32, t normalised per frame
-//       (ts - ts[0]) / (ts[-1] - ts[0] + 1e-6) in float32 arithmetic, as torch evaluates it.
+//       (ts - ts[0]) / (ts[-1] - ts[0] + 1e-6) in float32 arithmetic, as torch evaluates it;
+//   H5Dataset.augment_event + SequenceDataset's paused frames   dataloader/h5dataset.py:652-670, 769-789: per-frame flips
+//       and the zero event of a paused frame, applied in registers during the same gather.
 #include "common.cuh"
 
 namespace esr {
@@ -30,24 +32,42 @@ k_ts_search(const double *__restrict__ ts, long long n, const double *__restrict
     }
 }
 
-// one block per frame: events [start[f], start[f] + len[f]) of the columns -> out[off[f] ...] as fp32
+// one block per frame: events [start[f], start[f] + len[f]) of the columns -> out[off[f] ...] as fp32.
+// xform (optional) = one word per frame, H5Dataset.augment_event (h5dataset.py:652-670) and SequenceDataset's pause
+// (h5dataset.py:780-784, 317-319):
+//   bit 0: x -> W - 1 - x, bit 1: y -> H - 1 - y, bit 2: p -> -p  (the reference flips the float64 values before the fp32 cast;
+//          for int16 coordinates and W, H < 2^23 both sides are exact integers, so one fp32 subtraction gives the same bits);
+//   bit 3: paused, every output event is (x, y, t, p) = 0 (torch.zeros([4, 1]) for the one slot the host reserves); start ignored.
 __global__ void __launch_bounds__(256)
 k_gather_events(const short *__restrict__ xs, const short *__restrict__ ys, const double *__restrict__ ts,
                 const double *__restrict__ ps, const long long *__restrict__ start, const long long *__restrict__ off,
+                const int *__restrict__ xform, float wm1, float hm1,
                 float *__restrict__ oxs, float *__restrict__ oys, float *__restrict__ ots, float *__restrict__ ops)
 {
     const int f = blockIdx.x;
-    const long long s = start[f], o = off[f], n = off[f + 1] - o;
+    const int xf = xform ? xform[f] : 0;
+    const bool paused = xf & 8;
+    const long long s = paused ? 0 : start[f], o = off[f], n = off[f + 1] - o;
     float t0 = 0.f, den = 1.f;
-    if (ots && n > 0) {
+    if (ots && n > 0 && !paused) {
         t0 = (float)ts[s];
         den = __fadd_rn(__fsub_rn((float)ts[s + n - 1], t0), 1e-6f);          // fp32, like the torch expression
     }
     for (long long i = (long long)blockIdx.y * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.y * blockDim.x) {
-        oxs[o + i] = (float)xs[s + i];
-        oys[o + i] = (float)ys[s + i];
-        ops[o + i] = (float)ps[s + i];
-        if (ots) ots[o + i] = __fdiv_rn(__fsub_rn((float)ts[s + i], t0), den);
+        float x = 0.f, y = 0.f, p = 0.f, t = 0.f;
+        if (!paused) {
+            x = (float)xs[s + i];
+            y = (float)ys[s + i];
+            p = (float)ps[s + i];
+            if (xf & 1) x = __fsub_rn(wm1, x);
+            if (xf & 2) y = __fsub_rn(hm1, y);
+            if (xf & 4) p = -p;
+            if (ots) t = __fdiv_rn(__fsub_rn((float)ts[s + i], t0), den);
+        }
+        oxs[o + i] = x;
+        oys[o + i] = y;
+        ops[o + i] = p;
+        if (ots) ots[o + i] = t;
     }
 }
 
@@ -65,17 +85,26 @@ extern "C" int esr_ts_search(const double *ts, int64_t n, const double *queries,
     return ESR_OK;
 }
 
-extern "C" int esr_gather_events(const int16_t *xs, const int16_t *ys, const double *ts, const double *ps, const int64_t *start,
-                                 const int64_t *off, int n_frames, int64_t max_len, float *out_xs, float *out_ys, float *out_ts,
-                                 float *out_ps, esr_stream_t stream)
+extern "C" int esr_gather_events_aug(const int16_t *xs, const int16_t *ys, const double *ts, const double *ps, const int64_t *start,
+                                     const int64_t *off, const int32_t *xform, int W, int H, int n_frames, int64_t max_len,
+                                     float *out_xs, float *out_ys, float *out_ts, float *out_ps, esr_stream_t stream)
 {
     ESR_REQUIRE(xs && ys && ps && start && off && out_xs && out_ys && out_ps && n_frames >= 0, "esr_gather_events: bad arguments");
     ESR_REQUIRE(!out_ts || ts, "esr_gather_events: out_ts needs the ts column");
+    ESR_REQUIRE(!xform || (W > 0 && H > 0 && W < (1 << 23) && H < (1 << 23)), "esr_gather_events_aug: bad flip resolution");
     if (n_frames == 0) return ESR_OK;
     ESR_REQUIRE(n_frames <= 0x7fffffff, "esr_gather_events: too many frames");
     const unsigned gy = (unsigned)max((int64_t)1, min((int64_t)64, (max_len + 2047) / 2048));
     k_gather_events<<<dim3((unsigned)n_frames, gy), 256, 0, (cudaStream_t)stream>>>(xs, ys, ts, ps, (const long long *)start, (const long long *)off,
+                                                                                (const int *)xform, (float)(W - 1), (float)(H - 1),
                                                                                 out_xs, out_ys, out_ts, out_ps);
     ESR_LAUNCH_CHECK();
     return ESR_OK;
+}
+
+extern "C" int esr_gather_events(const int16_t *xs, const int16_t *ys, const double *ts, const double *ps, const int64_t *start,
+                                 const int64_t *off, int n_frames, int64_t max_len, float *out_xs, float *out_ys, float *out_ts,
+                                 float *out_ps, esr_stream_t stream)
+{
+    return esr_gather_events_aug(xs, ys, ts, ps, start, off, nullptr, 0, 0, n_frames, max_len, out_xs, out_ys, out_ts, out_ps, stream);
 }

@@ -14,15 +14,19 @@ At the GPU pipeline's speed that loader is the limiter.  Here:
     with the ground-truth alignment of `get_gt_event_indices_num` (h5dataset.py:196-262, 451-475).  Every timestamp lookup of
     a table is ONE batched launch of esr_ts_search, which reproduces the reference's bisection (exact hit returns the probed
     index, base_dataset.py:78-91 = binary_search.pyx:17-38) bit for bit.
-  * `SequenceReader` -- SequenceDataset's frame selection (h5dataset.py:729-791, pauses off) for a BATCH of sequences:
-    per-frame slices are gathered from the columns by one kernel launch per event stream (esr_gather_events: int16 / float64
-    -> fp32 SoA + frame offsets) and scattered by esr_b200.encodings.encode_frames into the three frame banks the scripts
-    read, returned in the window layout of HDF5DataLoaderSequence.custom_collate (esr_b200.dataset.collate_sequence's
-    output format) -- no per-frame Python, no per-frame H2D copy.
+  * `SequenceReader` -- SequenceDataset's frame selection (h5dataset.py:729-791) for a BATCH of sequences, with the
+    training loader's event flips (`data_augment`, h5dataset.py:282-288, 652-670) and random pauses (`sequence.pause`,
+    h5dataset.py:769-789): per-frame slices are gathered from the columns by one kernel launch per event stream
+    (esr_gather_events_aug: int16 / float64 -> fp32 SoA + frame offsets, flips and pauses applied in registers) and scattered
+    by esr_b200.encodings.encode_frames into the three frame banks the scripts read, returned in the window layout of
+    HDF5DataLoaderSequence.custom_collate (esr_b200.dataset.collate_sequence's output format) -- no per-frame Python, no
+    per-frame H2D copy.  The random decisions come from `draw_decisions`, which replays the reference's calls on the
+    module-level `random` generator (see there).
 There is no CPU fallback for the indexing / gather: they are C-ABI calls on a CUDA device.
 """
 import json
 import os
+import random
 
 import numpy as np
 import torch
@@ -203,17 +207,114 @@ class WindowIndex:
         return self.length
 
 
+FLIP_X, FLIP_Y, NEGATE_P, PAUSED = 1, 2, 4, 8        # the transform word of esr_gather_events_aug
+_EVENT_FLIPS = {"Horizontal": (0, FLIP_X), "Vertical": (1, FLIP_Y), "Polarity": (2, NEGATE_P)}   # name -> (seed offset, bit)
+
+
+def augmentation_enabled(config):
+    """True when load_batch draws random decisions: `data_augment.enabled` or `sequence.pause.enabled` (a missing key is off)."""
+    return bool(config.get("data_augment", {}).get("enabled", False) or
+                config.get("sequence", {}).get("pause", {}).get("enabled", False))
+
+
+def draw_decisions(config, n, L):
+    """The random decisions of n consecutive SequenceDataset.__getitem__ calls of L frames each, drawn from the module-level
+    `random` generator as the reference draws them, leaving the generator where the reference leaves it (the next
+    sequence's seed depends on that).  The reference's calls:
+
+      seed = random.randint(0, 2**32) per sequence (h5dataset.py:761);
+      per item (h5dataset.py:282-314): augment_event for the input and, with need_gt_events, the ground-truth events, then
+          augment_frame with need_gt_frame and again with mode == 'frame'; every mechanism reseeds (Horizontal: seed,
+          Vertical: seed + 1, Polarity: seed + 2; augment_frame skips Polarity) and draws once; a flip happens when that draw
+          is below the mechanism's augment_prob; unknown names are skipped;
+      per frame 1..L-1, before its item: u = random.random(), paused = u < (p_paused if paused else p_running) (:769-789).
+
+    random.seed replaces the whole generator state, so an item that reseeds at all leaves the generator exactly as its LAST
+    reseed and the draw after it do, whatever came before.  Hence, with augmentation on, every pause draw of a sequence is
+    the second value of that last stream: a sequence either pauses from frame 1 on or never does, and which reseed comes
+    last (set by the augment list, need_gt_events, need_gt_frame and mode) decides it.  This function uses that: the flips
+    and the pause draw come from private generators seeded as the reference seeds the global one, and the global generator
+    gets the sequence's randint and, at its end, the last item's reseed and draw; the reference's ~6 reseeds per frame cost
+    milliseconds per batch.  Items that never reseed (augmentation off) leave the pause draws successive values of the
+    global stream, drawn here from it directly.
+
+    -> {"seed": int64 [n], "flips": int32 [n] (FLIP_X | FLIP_Y | NEGATE_P bits; the same for every frame and for input and
+    ground truth), "paused": bool [n, L]}."""
+    aug = config.get("data_augment", {})
+    mechs = list(aug.get("augment", [])) if aug.get("enabled", False) else []
+    probs = aug.get("augment_prob", [])
+    pause = config.get("sequence", {}).get("pause", {})
+    pause_on = pause.get("enabled", False)
+    p_run, p_paused = pause.get("proba_pause_when_running"), pause.get("proba_pause_when_paused")
+    # the seed offset of an item's last reseed: augment_event's last known mechanism, unless augment_frame runs after it
+    last = None
+    for m in mechs:
+        if m in _EVENT_FLIPS:
+            last = _EVENT_FLIPS[m][0]
+    if config.get("need_gt_frame", False) or config["mode"] == "frame":
+        for m in mechs:
+            if m in ("Horizontal", "Vertical"):
+                last = _EVENT_FLIPS[m][0]
+
+    seeds, flips, paused = np.zeros(n, np.int64), np.zeros(n, np.int32), np.zeros((n, L), bool)
+    for s in range(n):
+        seed = random.randint(0, 2**32)
+        seeds[s] = seed
+        bits = 0
+        for i, m in enumerate(mechs):                    # augment_event; input and ground truth flip alike
+            if m in _EVENT_FLIPS:
+                off, bit = _EVENT_FLIPS[m]
+                if random.Random(seed + off).random() < probs[i]:
+                    bits ^= bit
+        flips[s] = bits
+        if last is not None:
+            tail = random.Random(seed + last)
+            tail.random()
+            u = tail.random()                            # every pause draw of this sequence
+        p = False
+        for f in range(1, L):
+            if pause_on:
+                if last is None:
+                    u = random.random()
+                p = u < (p_paused if p else p_run)
+            paused[s, f] = p
+        if last is not None:                             # the state the sequence's last item leaves behind
+            random.seed(seed + last)
+            random.random()
+    return {"seed": seeds, "flips": flips, "paused": paused}
+
+
+def frame_plan(decisions, seq_indices, step_size):
+    """draw_decisions' output for sequences seq_indices -> (dataset index of every frame [B * L], input transform words,
+    ground-truth transform words).  A paused frame re-reads index j + k of the last running frame (h5dataset.py:780-789):
+    its input becomes the one zero event; its ground truth stays that index's events, flipped like the rest of the sequence."""
+    paused = decisions["paused"]
+    L = paused.shape[1]
+    frames = np.asarray(seq_indices, np.int64)[:, None] * step_size + np.cumsum(~paused, axis=1) - 1
+    gt_xf = np.repeat(decisions["flips"], L).astype(np.int32)
+    inp_xf = gt_xf | np.where(paused.reshape(-1), PAUSED, 0).astype(np.int32)
+    return frames.reshape(-1), inp_xf, gt_xf
+
+
 class SequenceReader:
-    """Batched SequenceDataset (h5dataset.py:729-791; pause.enabled = False) + custom_collate on the GPU."""
+    """Batched SequenceDataset (h5dataset.py:729-791) + custom_collate on the GPU.
+
+    With `data_augment` or `sequence.pause` enabled, load_batch draws its random decisions from the module-level `random`
+    generator exactly as the reference's DataLoader(num_workers=0) would for the same sequences in the same order
+    (draw_decisions), and keeps them in `last_decisions`.  With both off it does not touch `random` and last_decisions is
+    None.  `add_noise` is not implemented (its noise comes from torch's CPU generator) and raises."""
 
     def __init__(self, store, config, where="pinned"):
+        if config.get("add_noise", {"enabled": False}).get("enabled", False):
+            raise _lib.ESRError("SequenceReader: add_noise (event noise from torch's CPU generator) is not implemented")
         self.index = WindowIndex(store, config)
+        self.config = config
         seq = config["sequence"]
         self.L = seq["sequence_length"]
         self.step_size = seq["step_size"] if seq.get("step_size") is not None else self.L
         assert self.L > 0 and self.step_size > 0
-        if seq.get("pause", {}).get("enabled", False):
-            raise _lib.ESRError("SequenceReader: random pauses are a training augmentation of the CPU loader, not implemented")
+        self.augmented = augmentation_enabled(config)
+        self.last_decisions = None
         if self.L >= self.index.length:
             self.length, self.L = 1, self.index.length
         else:
@@ -226,21 +327,32 @@ class SequenceReader:
     def __len__(self):
         return self.length
 
-    def _gather(self, cols, table, frames, need_ts=False):
-        """table [len, 2]; frames: flat list of dataset indices -> (xs, ys, ts|None, ps, off) CUDA fp32 SoA + int64 offsets."""
+    def _gather(self, cols, table, frames, xform=None, res=None, need_ts=False):
+        """table [len, 2]; frames: flat list of dataset indices; xform: int32 transform word per frame or None, flipping against
+        res = [H, W] -> (xs, ys, ts|None, ps, off) CUDA fp32 SoA + int64 offsets.  A PAUSED frame holds one zero event."""
         dev = _dev()
-        start = torch.from_numpy(np.ascontiguousarray(table[frames, 0]))
+        n = len(frames)
         lens = table[frames, 1] - table[frames, 0]
-        off = np.zeros(len(frames) + 1, dtype=np.int64)
-        off[1:] = np.cumsum(lens)
-        total, mx = int(off[-1]), int(lens.max(initial=1))
-        start_d, off_d = start.to(dev), torch.from_numpy(off).to(dev)
+        if xform is not None:
+            lens = np.where(xform & PAUSED, 1, lens)
+        # start [n] | off [n + 1] | xform [n] int32, packed so that one host-to-device copy carries them all
+        host = np.zeros(2 * n + 1 + (n + 1) // 2, dtype=np.int64)
+        host[:n] = table[frames, 0]
+        host[n + 1:2 * n + 1] = np.cumsum(lens)
+        if xform is not None:
+            host[2 * n + 1:].view(np.int32)[:n] = xform
+        total, mx = int(host[2 * n]), int(lens.max(initial=1))
+        d = torch.from_numpy(host).to(dev)
+        off_d = d[n:2 * n + 1]
+        xf_d = d[2 * n + 1:].view(torch.int32)[:n] if xform is not None else None
+        H, W = res if xform is not None else (0, 0)
         oxs, oys, ops = (torch.empty((max(total, 1),), dtype=torch.float32, device=dev) for _ in range(3))
         ots = torch.empty((max(total, 1),), dtype=torch.float32, device=dev) if need_ts else None
         with torch.cuda.device(dev):
-            _lib.check(_lib.lib().esr_gather_events(_lib.ptr(cols["xs"]), _lib.ptr(cols["ys"]), _lib.ptr(cols["ts"]), _lib.ptr(cols["ps"]),
-                                                    _lib.ptr(start_d), _lib.ptr(off_d), len(frames), mx, _lib.ptr(oxs), _lib.ptr(oys),
-                                                    _lib.ptr(ots), _lib.ptr(ops), _lib.stream_ptr()), "esr_gather_events")
+            _lib.check(_lib.lib().esr_gather_events_aug(_lib.ptr(cols["xs"]), _lib.ptr(cols["ys"]), _lib.ptr(cols["ts"]), _lib.ptr(cols["ps"]),
+                                                        _lib.ptr(d), _lib.ptr(off_d), _lib.ptr(xf_d), int(W), int(H), n, mx,
+                                                        _lib.ptr(oxs), _lib.ptr(oys), _lib.ptr(ots), _lib.ptr(ops), _lib.stream_ptr()),
+                       "esr_gather_events_aug")
         return oxs[:total], oys[:total], (ots[:total] if need_ts else None), ops[:total], off_d, mx
 
     def frames_of(self, seq_indices):
@@ -248,25 +360,36 @@ class SequenceReader:
 
     def load_batch(self, seq_indices):
         """-> the L - num_frame + 1 window dicts of custom_collate for sequences `seq_indices` ('inp_cnt', 'inp_scaled_cnt',
-        'gt_cnt' as [B, N, 2, ., .] views of frame banks, 'bank' = the [B, L, 2, ., .] banks for forward_sequence / train_step)."""
+        'gt_cnt' as [B, N, 2, ., .] views of frame banks, 'bank' = the [B, L, 2, ., .] banks for forward_sequence / train_step).
+        With augmentation or pauses enabled, the batch consumes the module-level `random` generator as the reference's loader
+        would for these sequences in this order; the decisions are kept in `last_decisions`."""
+        seq_indices = list(seq_indices)
         for i in seq_indices:
             assert 0 <= i < self.length
         B, L = len(seq_indices), self.L
-        frames = self.frames_of(seq_indices)
-        ix, iy, _, ip, ioff, imax = self._gather(self.inp_cols, self.index.event_indices, frames)
         H, W = self.inp_sensor_resolution
         kH, kW = self.gt_sensor_resolution
+        if self.augmented:
+            self.last_decisions = draw_decisions(self.config, B, L)
+            frames, inp_xf, gt_xf = frame_plan(self.last_decisions, seq_indices, self.step_size)
+        else:
+            frames, inp_xf, gt_xf = self.frames_of(seq_indices), None, None
+        ix, iy, _, ip, ioff, imax = self._gather(self.inp_cols, self.index.event_indices, frames, inp_xf, (H, W))
         inp_cnt = encodings.encode_frames(ix, iy, ip, ioff, None, (H, W), imax, sanitised=True).view(B, L, 2, H, W)
         inp_scaled = encodings.encode_frames(ix, iy, ip, ioff, (H, W), (kH, kW), imax, sanitised=True).view(B, L, 2, kH, kW)
         bank = {"inp_cnt": inp_cnt, "inp_scaled_cnt": inp_scaled}
         if self.gt_cols is not None:
-            gx, gy, _, gp, goff, gmax = self._gather(self.gt_cols, self.index.gt_event_indices, frames)
+            gx, gy, _, gp, goff, gmax = self._gather(self.gt_cols, self.index.gt_event_indices, frames, gt_xf, (kH, kW))
             bank["gt_cnt"] = encodings.encode_frames(gx, gy, gp, goff, None, (kH, kW), gmax, sanitised=True).view(B, L, 2, kH, kW)
         N = self.num_frame
         return [dict({k: v[:, w:w + N] for k, v in bank.items()}, bank=bank) for w in range(L - N + 1)]
 
-    def events_of_frame(self, frame, gt=False):
-        """One frame's formatted events [4, n] fp32 on the GPU = BaseDataset.event_formatting(H5Dataset.get_events(idx0, idx1))."""
+    def events_of_frame(self, frame, gt=False, xform=None):
+        """One frame's formatted events [4, n] fp32 on the GPU = BaseDataset.event_formatting(H5Dataset.get_events(idx0, idx1)),
+        with xform (a transform word of FLIP_X | FLIP_Y | NEGATE_P | PAUSED) = event_formatting(augment_event(...)) against the
+        stream's sensor resolution, or the zero event of a paused frame."""
         cols, table = (self.gt_cols, self.index.gt_event_indices) if gt else (self.inp_cols, self.index.event_indices)
-        xs, ys, ts, ps, _, _ = self._gather(cols, table, np.array([frame], dtype=np.int64), need_ts=True)
+        res = self.gt_sensor_resolution if gt else self.inp_sensor_resolution
+        xf = None if xform is None else np.array([xform], dtype=np.int32)
+        xs, ys, ts, ps, _, _ = self._gather(cols, table, np.array([frame], dtype=np.int64), xf, res, need_ts=True)
         return torch.stack([xs, ys, ts, ps])

@@ -302,11 +302,18 @@ int esr_metrics_planes(const float *pred, const float *tgt, int n_planes, int H,
  *   index, else the left insertion point); ts sorted float64 [n], device or host-mapped memory;
  *   H5Dataset.get_events / get_gt_events + BaseDataset.event_formatting (h5dataset.py:492-506, base_dataset.py:26-33):
  *   frame f = rows [start[f], start[f] + off[f+1] - off[f]) of the int16 x / y and float64 t / p columns -> fp32 SoA at
- *   out_*[off[f] ...]; out_ts (optional) = per-frame normalised time (ts - ts[0]) / (ts[-1] - ts[0] + 1e-6) in fp32. */
+ *   out_*[off[f] ...]; out_ts (optional) = per-frame normalised time (ts - ts[0]) / (ts[-1] - ts[0] + 1e-6) in fp32.
+ * esr_gather_events_aug adds H5Dataset.augment_event and SequenceDataset's pause (h5dataset.py:652-670, 769-789, 317-319) as one
+ * word per frame, xform[f] (device memory; NULL = esr_gather_events): bit 0 x -> W - 1 - x, bit 1 y -> H - 1 - y, bit 2 p -> -p,
+ * bit 3 paused: the frame's events are all (0, 0, 0, 0) (the host gives it length 1, the reference's torch.zeros([4, 1]))
+ * and start[f] is not read.  W, H: the stream's sensor resolution, 0 < W, H < 2^23 when xform is given. */
 int esr_ts_search(const double *ts, int64_t n, const double *queries, int64_t nq, int64_t *out, esr_stream_t stream);
 int esr_gather_events(const int16_t *xs, const int16_t *ys, const double *ts, const double *ps, const int64_t *start,
                       const int64_t *off, int n_frames, int64_t max_len, float *out_xs, float *out_ys, float *out_ts,
                       float *out_ps, esr_stream_t stream);
+int esr_gather_events_aug(const int16_t *xs, const int16_t *ys, const double *ts, const double *ps, const int64_t *start,
+                          const int64_t *off, const int32_t *xform, int W, int H, int n_frames, int64_t max_len,
+                          float *out_xs, float *out_ys, float *out_ts, float *out_ps, esr_stream_t stream);
 
 #ifdef __cplusplus
 }
