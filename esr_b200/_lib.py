@@ -52,6 +52,7 @@ class ConvDesc(ctypes.Structure):
 
 SIGNATURES.update({
     "esr_conv_tc": (c_int, [ctypes.POINTER(ConvDesc), c_void_p]),
+    "esr_conv_tc_chunked": (c_int, [ctypes.POINTER(ConvDesc), ctypes.POINTER(c_int), ctypes.POINTER(c_int), c_void_p]),
     "esr_conv_weight_bytes": (c_size_t, [c_int, c_int, c_int]),
     "esr_pack_conv_weight": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p]),
     "esr_split_from_nchw": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p]),
@@ -62,6 +63,8 @@ SIGNATURES.update({
 SIGNATURES.update({
     "esr_net_param_bytes": (c_size_t, []),
     "esr_net_pack_params": (c_int, [c_void_p, c_void_p, c_void_p]),
+    "esr_net_param_bytes_n": (c_size_t, [c_int]),
+    "esr_net_pack_params_n": (c_int, [c_int, c_void_p, c_void_p, c_void_p]),
     "esr_net_workspace_bytes": (c_size_t, [c_int, c_int, c_int, c_int, c_int]),
     "esr_net_create": (c_int, [ctypes.POINTER(c_void_p), c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_size_t, c_void_p]),
     "esr_net_destroy": (c_int, [c_void_p]),

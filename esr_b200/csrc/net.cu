@@ -1,6 +1,7 @@
 // net.cu -- DeepRecurrNet.forward (models/model.py:294-344) as a fixed launch sequence over the sm_90a kernels.
 //
-// A "net" is a plan for one (B, N=3, H, W): every intermediate tensor has a fixed place in a caller-provided
+// A "net" is a plan for one (B, N, L, H, W), N = num_frame any odd number >= 3: every intermediate tensor has a fixed place in a
+// caller-provided
 // workspace, every TMA tensor map / launch descriptor is built once at creation, and forward() only enqueues
 // kernels on the caller's stream (no allocation, no host synchronisation, CUDA-graph capturable).
 // Recurrent ConvGRU states (models/model.py:72,102-114) live in the workspace and persist across forward() calls
@@ -39,9 +40,12 @@ static const TLInfo TLS[T_COUNT] = {
     {P_GF_W, P_GF_B, -1, -1, 64, 128, 1}, {P_OF0_W, P_OF0_B, -1, -1, 64, 128, 3}, {P_OF1_W, P_OF1_B, -1, -1, 64, 64, 3},
     {P_COM_W, P_COM_B, -1, -1, 216, 64, 3}, {P_DCN_W, P_DCN_B, -1, -1, 64, 64, 3}, {P_CB0_W, P_CB0_B, -1, -1, 64, 128, 3},
     {P_CB1_W, P_CB1_B, -1, -1, 64, 64, 3}, {P_KER_W, P_KER_B, -1, -1, 2, 64, 1}, {P_DF0_W, P_DF0_B, -1, -1, 64, 128, 3},
-    {P_DF1_W, P_DF1_B, -1, -1, 64, 64, 3}, {P_DN0_W, P_DN0_B, -1, -1, 64, 192, 3}, {P_DN1_W, P_DN1_B, -1, -1, 64, 64, 3},
+    {P_DF1_W, P_DF1_B, -1, -1, 64, 64, 3}, {P_DN0_W, P_DN0_B, -1, -1, 64, 0, 3}, {P_DN1_W, P_DN1_B, -1, -1, 64, 64, 3},
     {P_AT0_W, P_AT0_B, -1, -1, 1, 64, 3}, {P_RC0_W, P_RC0_B, -1, -1, 32, 64, 3},
 };
+// input channels of a tensor-core layer: dense_fusion.0 reads cat(N-1 aligned neighbours, middle frame) = N x 64
+static int tl_cin(int t, int N) { return t == T_DN0 ? 64 * N : TLS[t].cin; }
+static bool num_frame_ok(int N) { return N >= 3 && N % 2 == 1 && N <= 255; }
 // direct (CUDA-core) layers
 enum DL : int { D_HEAD, D_ENC0, D_ENC1, D_ENC2, D_AT1, D_AT2, D_RC0, D_RC1, D_RC2, D_TAIL, D_COUNT };
 struct DLInfo { int w, b, cout, cin; DirectKind kind; };
@@ -60,14 +64,16 @@ struct ParamLayout {
     size_t nw_pm1, nw_at0, nw_ker;       // fp32 [tap][ci][co] weights of the narrow-output layers (conv_narrow)
     size_t total;
 };
-static const ParamLayout &param_layout()
+// Only dense_fusion.0's packed weight depends on N; the entries after it move with its size.  N = 3 is the layout of
+// esr_net_param_bytes() / esr_net_pack_params().
+static ParamLayout param_layout(int N)
 {
-    static ParamLayout L = [] {
-        ParamLayout l{};
+    ParamLayout l{};
+    {
         size_t off = 0;
         auto take = [&](size_t bytes) { size_t r = off; off = align_up(off + bytes, 256); return r; };
         for (int i = 0; i < T_COUNT; ++i) {
-            l.tw[i] = take(tc_packed_weight_bytes(TLS[i].cout, TLS[i].cin, TLS[i].k * TLS[i].k));
+            l.tw[i] = take(tc_packed_weight_bytes(TLS[i].cout, tl_cin(i, N), TLS[i].k * TLS[i].k));
             l.tb[i] = take(sizeof(float) * tc_npad(TLS[i].cout));
         }
         for (int i = 0; i < D_COUNT; ++i) {
@@ -79,9 +85,8 @@ static const ParamLayout &param_layout()
         l.fc1w = take(sizeof(float) * 128 * 32); l.fc1b = take(sizeof(float) * 128);
         l.nw_pm1 = take(sizeof(float) * 9 * 64); l.nw_at0 = take(sizeof(float) * 9 * 64); l.nw_ker = take(sizeof(float) * 64 * 2);
         l.total = off;
-        return l;
-    }();
-    return L;
+    }
+    return l;
 }
 
 // ---- the plan ---------------------------------------------------------------------------------------------------
@@ -92,6 +97,7 @@ static const ParamLayout &param_layout()
 struct Net {
     int B, N, L, Wn, VB, FR, H, W, Hc, Wc, h, w;
     int pad_top, pad_bottom, pad_left, pad_right;
+    ParamLayout P;  // layout of the packed blob for this N
     char *params;   // packed blob
     char *ws;       // workspace
     size_t ws_bytes;
@@ -100,7 +106,7 @@ struct Net {
     SplitTensor t_of0, t_off, cols, aligned, t_cb0, feat, ycat, t_df0, fused, t_dn0, x0, pre0, up0, x1, pre1, x2, pre2, x3;
     float *maps, *zbuf, *om, *sk, *mx, *ck, *att0, *att1, *att2;
     // index maps (device)
-    int *m_fr, *m_pairA, *m_pairB, *m_ltc5, *m_lf3res, *m_f0, *m_fm, *m_dn[3], *m_gf_f, *m_gf_r, *m_gfres;
+    int *m_fr, *m_pairA, *m_pairB, *m_ltc5, *m_lf3res, *m_f0, *m_fm, *m_gf_f, *m_gf_r, *m_gfres;
     std::vector<int *> m_gx, m_gh;     // per GRU step (Wn * N of them)
     // prepared tensor-core launches
     ConvTCArgs c_pm0, c_pm1, c_lf1, c_lf2, c_lf3, c_gx, c_gf, c_of0, c_of1, c_com, c_dcn, c_cb0, c_cb1, c_ker, c_df0, c_df1,
@@ -177,7 +183,6 @@ static size_t layout(Net &n)
     n.m_fr = ints(VN);
     n.m_pairA = ints(np); n.m_pairB = ints(np); n.m_ltc5 = ints((size_t)VN * 5); n.m_lf3res = ints(VN);
     n.m_f0 = ints(nf); n.m_fm = ints(nf);
-    for (int k = 0; k < 3; ++k) n.m_dn[k] = ints(VB);
     n.m_gf_f = ints(VN); n.m_gf_r = ints(VN); n.m_gfres = ints(VN);
     n.m_gx.resize(nsteps); n.m_gh.resize(nsteps);
     for (int s = 0; s < nsteps; ++s) { n.m_gx[s] = ints(2 * B); n.m_gh[s] = ints(2 * B); }
@@ -191,8 +196,8 @@ static int upload(int *dst, const std::vector<int> &v, cudaStream_t st)
     return ESR_OK;
 }
 
-static const void *pw(const Net &n, int t) { return n.params + param_layout().tw[t]; }
-static const float *pb(const Net &n, int t) { return (const float *)(n.params + param_layout().tb[t]); }
+static const void *pw(const Net &n, int t) { return n.params + n.P.tw[t]; }
+static const float *pb(const Net &n, int t) { return (const float *)(n.params + n.P.tb[t]); }
 
 static ConvTCDesc mk(const Net &n, int t, int n_img, int act)
 {
@@ -247,11 +252,6 @@ static int build(Net &n, cudaStream_t st)
             ++k;
         }
         if ((rc = upload(n.m_f0, f0, st)) || (rc = upload(n.m_fm, fm, st))) return rc;
-        for (int kk = 0; kk < 3; ++kk) {
-            std::vector<int> m(VB);
-            for (int vb = 0; vb < VB; ++vb) m[vb] = kk < N - 1 ? kk * VB + vb : vb * N + mid;
-            if ((rc = upload(n.m_dn[kk], m, st))) return rc;
-        }
         // GRU: global step g = w*N + s reads state slot g and writes slot g+1 (slot 0 = carried state)
         std::vector<int> gf(VN), gr(VN);
         for (int vb = 0; vb < VB; ++vb) {
@@ -333,8 +333,11 @@ static int build(Net &n, cudaStream_t st)
     if ((rc = conv_tc_prepare(d, &n.c_df0))) return rc;
     d = mk(n, T_DF1, nf, ACT_NONE); d.src[0] = n.t_df0; d.out = n.fused;
     if ((rc = conv_tc_prepare(d, &n.c_df1))) return rc;
-    d = mk(n, T_DN0, VB, ACT_RELU); d.n_src = 3;
-    d.src[0] = n.fused; d.src_img[0] = n.m_dn[0]; d.src[1] = n.fused; d.src_img[1] = n.m_dn[1]; d.src[2] = n.tp; d.src_img[2] = n.m_dn[2];
+    // dense_fusion.0 over cat(fused_0 .. fused_{N-2}, middle frame) without materialising the concatenation: `fused` holds the N-1
+    // neighbours k-major (image k * VB + vb), so it is one source of N-1 chunks VB images apart; the first VB entries of m_fm
+    // map window vb to its middle frame
+    d = mk(n, T_DN0, VB, ACT_RELU); d.n_src = 2;
+    d.src[0] = n.fused; d.src_chunks[0] = N - 1; d.chunk_img_step[0] = VB; d.src[1] = n.tp; d.src_img[1] = n.m_fm;
     d.out = n.t_dn0;
     if ((rc = conv_tc_prepare(d, &n.c_dn0))) return rc;
     d = mk(n, T_DN1, VB, ACT_NONE); d.src[0] = n.t_dn0; d.out = n.x0;
@@ -346,7 +349,7 @@ static int build(Net &n, cudaStream_t st)
     if ((rc = conv_tc_prepare(d, &n.c_rc0))) return rc;
 
     // ---------------- direct launches
-    const ParamLayout &Lp = param_layout();
+    const ParamLayout &Lp = n.P;
     auto base = [&](int i, int act) {
         DirectArgs a; a.w = (const float *)(n.params + Lp.dw[i]); a.bias = (const float *)(n.params + Lp.db[i]); a.act = act;
         a.w_mma = n.params + Lp.dm[i];
@@ -425,7 +428,7 @@ static int forward(Net &n, const float *input, const int *in_img, float *output,
 #define RUNT(name_, args) RUNC(name_, PC_TC, tc_flops(args), tc_bytes(args), conv_tc_launch(args, st))
 #define RUND(name_, kind, dl, args) RUNC(name_, PC_DIRECT, direct_flops(dl, args), direct_bytes(dl, args), conv_direct(kind, args, st))
     const int B = n.B, N = n.N, VB = n.VB, VN = VB * N, nf = (N - 1) * VB, nsteps = n.Wn * N;
-    const ParamLayout &L = param_layout();
+    const ParamLayout &L = n.P;
     // Cout <= 2 layers on CUDA cores (elementwise.cu conv_narrow).  Measured (profiles/r2_notes.md): only the 1x1 spatial-attention
     // kernel wins (18.8 -> 14.8 us); the 3x3 ones are latency-bound there (pred_map[1] 41 -> 51, tail 66 -> 93 us) and stay on the
     // tensor-core / mma.sync kernels.  ESR_NARROW_ALL=1 routes all of them through conv_narrow, ESR_NARROW_TC=1 none.
@@ -532,20 +535,23 @@ static void net_dims(Net &n, int B, int N, int L, int H, int W)
     n.pad_left = (n.Wc - W + 1) / 2; n.pad_right = (n.Wc - W) / 2;
 }
 
-extern "C" size_t esr_net_param_bytes(void) { return param_layout().total; }
+extern "C" size_t esr_net_param_bytes_n(int num_frame) { return num_frame_ok(num_frame) ? param_layout(num_frame).total : 0; }
+extern "C" size_t esr_net_param_bytes(void) { return esr_net_param_bytes_n(3); }
 
-extern "C" int esr_net_pack_params(const float *const *p, void *blob, esr_stream_t stream)
+extern "C" int esr_net_pack_params_n(int num_frame, const float *const *p, void *blob, esr_stream_t stream)
 {
     ESR_REQUIRE(p && blob, "esr_net_pack_params: null pointer");
+    ESR_REQUIRE(num_frame_ok(num_frame), "esr_net_pack_params: num_frame=%d (odd, >= 3)", num_frame);
     cudaStream_t st = (cudaStream_t)stream;
-    const ParamLayout &L = param_layout();
+    const ParamLayout L = param_layout(num_frame);
     char *out = (char *)blob;
     int rc;
     ESR_CUDA_CHECK(cudaMemsetAsync(blob, 0, L.total, st));
     for (int i = 0; i < T_COUNT; ++i) {
         const TLInfo &t = TLS[i];
         const int co_each = t.w2 >= 0 ? t.cout / 2 : t.cout;
-        if ((rc = pack_conv_weight2(p[t.w], t.w2 >= 0 ? p[t.w2] : nullptr, co_each, t.cin, t.k, out + L.tw[i], st))) return rc;
+        if ((rc = pack_conv_weight2(p[t.w], t.w2 >= 0 ? p[t.w2] : nullptr, co_each, tl_cin(i, num_frame), t.k, out + L.tw[i], st)))
+            return rc;
         ESR_CUDA_CHECK(cudaMemcpyAsync(out + L.tb[i], p[t.b], sizeof(float) * co_each, cudaMemcpyDeviceToDevice, st));
         if (t.b2 >= 0)
             ESR_CUDA_CHECK(cudaMemcpyAsync(out + L.tb[i] + sizeof(float) * co_each, p[t.b2], sizeof(float) * co_each,
@@ -566,6 +572,24 @@ extern "C" int esr_net_pack_params(const float *const *p, void *blob, esr_stream
     if ((rc = pack_narrow_weight(p[P_KER_W], 2, 1, (float *)(out + L.nw_ker), st))) return rc;
     return ESR_OK;
 }
+extern "C" int esr_net_pack_params(const float *const *p, void *blob, esr_stream_t stream) { return esr_net_pack_params_n(3, p, blob, stream); }
+
+// bytes from `p` to the end of the device allocation holding it (0 = unknown): a blob packed for a smaller num_frame is too short
+static size_t bytes_to_allocation_end(const void *p)
+{
+    typedef CUresult (*PFN_range)(CUdeviceptr *, size_t *, CUdeviceptr);
+    static PFN_range fn = [] {
+        void *f = nullptr;
+        cudaDriverEntryPointQueryResult q;
+        if (cudaGetDriverEntryPoint("cuMemGetAddressRange", &f, cudaEnableDefault, &q) != cudaSuccess || q != cudaDriverEntryPointSuccess)
+            f = nullptr;
+        return (PFN_range)f;
+    }();
+    CUdeviceptr base = 0;
+    size_t size = 0;
+    if (!fn || fn(&base, &size, (CUdeviceptr)p) != CUDA_SUCCESS) return 0;
+    return (size_t)(base + size - (CUdeviceptr)p);
+}
 
 extern "C" size_t esr_net_workspace_bytes(int B, int N, int L, int H, int W)
 {
@@ -582,9 +606,16 @@ extern "C" int esr_net_create(esr_net_t *out, int B, int N, int L, int H, int W,
     ESR_REQUIRE(out && params && workspace, "esr_net_create: null pointer");
     ESR_REQUIRE(B > 0 && H > 0 && W > 0 && L >= N, "esr_net_create: bad dims");
     ESR_REQUIRE(2 * B <= 65535 && (long long)B * L * ((H + 7) / 8) * ((W + 7) / 8) < (1ll << 28), "esr_net_create: batch too large");
-    if (N != 3) { set_error("esr_net_create: num_frame=%d (only the shipped num_frame=3 is implemented)", N); return ESR_EUNSUPPORTED; }
+    if (!num_frame_ok(N)) { set_error("esr_net_create: num_frame=%d (the reference needs an odd num_frame >= 3)", N); return ESR_EUNSUPPORTED; }
+    const size_t blob_room = bytes_to_allocation_end(params);
+    if (blob_room != 0 && blob_room < esr_net_param_bytes_n(N)) {
+        set_error("esr_net_create: the parameter blob (%zu bytes to the end of its allocation) is smaller than the %zu bytes of "
+                  "num_frame=%d; pack it with esr_net_pack_params_n(%d, ...)", blob_room, esr_net_param_bytes_n(N), N, N);
+        return ESR_EINVAL;
+    }
     Net *n = new Net();
     net_dims(*n, B, N, L, H, W);
+    n->P = param_layout(N);
     n->params = (char *)params; n->ws = (char *)workspace; n->ws_bytes = ws_bytes;
     const size_t need = layout(*n);
     if (need > ws_bytes) { set_error("esr_net_create: workspace %zu < %zu", ws_bytes, need); delete n; return ESR_EWORKSPACE; }

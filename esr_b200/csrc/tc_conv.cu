@@ -6,7 +6,9 @@
 //   (64 ch, TW, TH, 1 image, 1 plane) taken at the tap's (dy, dx) shift; out-of-image coordinates are zero-filled
 //   by TMA, which is exactly the conv's zero padding.  The box lands in shared memory in the 128B-swizzled K-major
 //   layout that wgmma reads, so no thread touches the operands.
-// * Channel concatenation (torch.cat in the reference) is a K-split over up to 3 source tensors.
+// * Channel concatenation (torch.cat in the reference) is a K-split over up to 3 source tensors.  A 64-channel source can also
+//   stand for several chunks, chunk j at image + j * step (the num_frame-way concatenation of dense_fusion): one multiply-add
+//   in the producer per K-block.
 // * fp32 parity: three bf16 MMAs per K-step (lo*hi + hi*lo + hi*hi) accumulate in fp32 registers => ~2^-17 relative
 //   operand error instead of bf16's 2^-9 (the reference network is fp32-only).
 // * Warp roles: warps 0-7 = two consumer warpgroups (pixel rows 0-63 / 64-127 of the tile, accumulators in registers,
@@ -86,11 +88,12 @@ __device__ __forceinline__ void conv_tiles(const ConvTCArgs &a, int tile0, int s
                     const int gchunk = kb / a.ntaps, tap = kb - gchunk * a.ntaps;
                     while (gchunk >= a.chunk_end[src]) { chunk_base = a.chunk_end[src]; ++src; }
                     const int dy = a.ntaps == 9 ? tap / 3 - 1 : 0, dx = a.ntaps == 9 ? tap % 3 - 1 : 0;
-                    const int simg = a.src_img[src] ? a.src_img[src][img] : img;
+                    const int cc = gchunk - chunk_base, istep = a.chunk_img_step[src];
+                    const int simg = (a.src_img[src] ? a.src_img[src][img] : img) + cc * istep;
                     mbar_wait(m.bar_empty + 8u * s, ph ^ 1u);
                     mbar_expect_tx(m.bar_full + 8u * s, tx_bytes);
                     const uint32_t st = m.ring + s * m.stage_stride;
-                    const int c0 = (gchunk - chunk_base) * 64;
+                    const int c0 = istep ? 0 : cc * 64;
                     tma_load_5d(&a.amap[src], m.bar_full + 8u * s, st, c0, x0 + dx, y0 + dy, simg, 0);
                     tma_load_5d(&a.amap[src], m.bar_full + 8u * s, st + TC_A_BYTES, c0, x0 + dx, y0 + dy, simg, 1);
                     tma_load_3d(&a.bmap, m.bar_full + 8u * s, st + 2u * TC_A_BYTES, 0, 0, kb);
@@ -275,8 +278,16 @@ int conv_tc_prepare(const ConvTCDesc &d, ConvTCArgs *args)
     for (int s = 0; s < d.n_src; ++s) {
         const SplitTensor &t = d.src[s];
         ESR_REQUIRE(t.base && t.C % 64 == 0 && t.H == H && t.W == W, "conv_tc: source %d has C=%d H=%d W=%d", s, t.C, t.H, t.W);
-        chunks += t.C / 64;
+        if (d.chunk_img_step[s] != 0) {
+            ESR_REQUIRE(t.C == 64 && d.src_chunks[s] >= 1, "conv_tc: source %d with an image step needs C=64 and src_chunks >= 1", s);
+            chunks += d.src_chunks[s];
+        } else {
+            ESR_REQUIRE(d.src_chunks[s] == 0 || d.src_chunks[s] == t.C / 64, "conv_tc: source %d has %d chunks, not %d", s, t.C / 64,
+                        d.src_chunks[s]);
+            chunks += t.C / 64;
+        }
         a.chunk_end[s] = chunks;
+        a.chunk_img_step[s] = d.chunk_img_step[s];
         a.src_img[s] = d.src_img[s];
         int rc = make_amap(t, TW, TH, &a.amap[s]);
         if (rc) return rc;
@@ -536,7 +547,7 @@ static SplitTensor mk_split(const void *p, int n_img, int H, int W, int C)
     return t;
 }
 
-extern "C" int esr_conv_tc(const esr_conv_desc *c, esr_stream_t stream)
+static int conv_tc_abi(const esr_conv_desc *c, const int *src_chunks, const int *chunk_img_step, esr_stream_t stream)
 {
     ESR_REQUIRE(c, "esr_conv_tc: null descriptor");
     ConvTCDesc d;
@@ -544,6 +555,8 @@ extern "C" int esr_conv_tc(const esr_conv_desc *c, esr_stream_t stream)
     for (int s = 0; s < c->n_src && s < TC_MAX_SRC; ++s) {
         d.src[s] = mk_split(c->src[s], c->src_n_img[s], c->H, c->W, c->src_C[s]);
         d.src_img[s] = c->src_img[s];
+        if (src_chunks) d.src_chunks[s] = src_chunks[s];
+        if (chunk_img_step) d.chunk_img_step[s] = chunk_img_step[s];
     }
     d.ntaps = c->ntaps; d.cout = c->cout; d.wpacked = c->wpacked; d.bias = c->bias; d.n_img = c->n_img;
     d.act = c->act; d.act_from = c->act_from; d.res_mode = c->res_mode; d.epi_mode = c->epi_mode;
@@ -556,6 +569,11 @@ extern "C" int esr_conv_tc(const esr_conv_desc *c, esr_stream_t stream)
     int rc = conv_tc_prepare(d, &args);
     if (rc) return rc;
     return conv_tc_launch(args, (cudaStream_t)stream);
+}
+extern "C" int esr_conv_tc(const esr_conv_desc *c, esr_stream_t stream) { return conv_tc_abi(c, nullptr, nullptr, stream); }
+extern "C" int esr_conv_tc_chunked(const esr_conv_desc *c, const int *src_chunks, const int *chunk_img_step, esr_stream_t stream)
+{
+    return conv_tc_abi(c, src_chunks, chunk_img_step, stream);
 }
 extern "C" size_t esr_conv_weight_bytes(int cout, int cin, int ksz) { return tc_packed_weight_bytes(cout, cin, ksz * ksz); }
 extern "C" int esr_pack_conv_weight(const float *w0, const float *w1, int cout_each, int cin, int ksz, void *dst, esr_stream_t st)

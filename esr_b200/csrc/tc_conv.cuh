@@ -39,6 +39,9 @@ struct ConvTCArgs {
     // GRU extras
     const __nv_bfloat16 *h_prev; size_t h_plane;                  // [*,H,W,64] split
     float *z_buf;                                                 // [n_img,H,W,64] fp32 (ZR writes, OUT reads)
+    // 0: chunk c of source s is channels 64 (c - chunk base); k != 0: channels 0-63 of image src_img + (c - chunk base) * k.
+    // Last, so that the offsets of the fields above (and the register allocation of every k_conv_tc instantiation) do not move.
+    int chunk_img_step[TC_MAX_SRC];
 };
 
 static_assert(sizeof(ConvTCArgs) <= 1024, "ConvTCArgs: keep the kernel argument block within 1 KB");
@@ -47,6 +50,11 @@ static_assert(sizeof(ConvTCArgs) <= 1024, "ConvTCArgs: keep the kernel argument 
 struct ConvTCDesc {
     SplitTensor src[TC_MAX_SRC];
     const int *src_img[TC_MAX_SRC] = {nullptr, nullptr, nullptr};
+    // A source with chunk_img_step[s] = k != 0 is a 64-channel tensor that contributes src_chunks[s] chunks: chunk j reads image
+    // src_img[s][img] + j * k.  This concatenates images of one tensor along channels without materialising the concatenation
+    // (dense_fusion's N-1 aligned neighbours, stored k-major).  The caller keeps the last image inside the tensor.
+    int src_chunks[TC_MAX_SRC] = {0, 0, 0};
+    int chunk_img_step[TC_MAX_SRC] = {0, 0, 0};
     int n_src = 1;
     int ntaps = 9;                  // 9 (3x3, pad 1) or 1 (1x1)
     int cout = 64;

@@ -54,8 +54,10 @@ def pad_bias(b, cout):
 
 def conv_tc(srcs, wpacked, bias, cout, ntaps=9, act=None, act_from=0, src_img=None, n_img=None,
             res=None, res_mode=0, res_img=None, out=None, out_coff=0, out_f32=None,
-            epi_mode=0, h_prev=None, z_buf=None):
-    """Runs one tensor-core convolution.  srcs: list of Split; returns (out Split or None, out_f32 or None)."""
+            epi_mode=0, h_prev=None, z_buf=None, src_chunks=None, chunk_img_step=None):
+    """Runs one tensor-core convolution.  srcs: list of Split; returns (out Split or None, out_f32 or None).
+    chunk_img_step[i] = k != 0: the 64-channel source i stands for src_chunks[i] chunks, chunk j read from image
+    src_img[i][img] + j * k (esr_conv_tc_chunked)."""
     d = _lib.ConvDesc()
     keep = []
     H, W = srcs[0].H, srcs[0].W
@@ -87,6 +89,11 @@ def conv_tc(srcs, wpacked, bias, cout, ntaps=9, act=None, act_from=0, src_img=No
         d.h_prev, d.h_n_img = h_prev.buf.data_ptr(), h_prev.n_img
     if z_buf is not None:
         d.z_buf = z_buf.data_ptr()
-    _lib.check(_lib.lib().esr_conv_tc(ctypes.byref(d), _lib.stream_ptr()), "esr_conv_tc")
+    if chunk_img_step is None:
+        _lib.check(_lib.lib().esr_conv_tc(ctypes.byref(d), _lib.stream_ptr()), "esr_conv_tc")
+    else:
+        chunks = (ctypes.c_int * 3)(*(list(src_chunks) + [0] * (3 - len(src_chunks))))
+        steps = (ctypes.c_int * 3)(*(list(chunk_img_step) + [0] * (3 - len(chunk_img_step))))
+        _lib.check(_lib.lib().esr_conv_tc_chunked(ctypes.byref(d), chunks, steps, _lib.stream_ptr()), "esr_conv_tc_chunked")
     torch.cuda.current_stream().synchronize() if keep else None
     return out, out_f32

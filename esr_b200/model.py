@@ -108,7 +108,7 @@ class _STFusion(nn.Module):
 
 
 class _Plan:
-    """One esr_net_t for a (B, L, H, W, device) with its workspace (L = 3: the reference's single-window forward)."""
+    """One esr_net_t for a (B, L, H, W, device) with its workspace (L = num_frame: the reference's single-window forward)."""
 
     def __init__(self, B, N, L, H, W, blob, device):
         lib = _lib.lib()
@@ -152,12 +152,14 @@ class DeepRecurrNet(nn.Module):
     # ------------------------------------------------------------------------------------------
     def _check_supported(self):
         c = self._cfg
-        ok = (c["inch"] == 2 and c["basech"] == 8 and c["num_frame"] == 3 and c["norm"] is None and c["activation"] == "relu"
-              and c["has_ltc"] and c["has_gtc"] and not c["gtc_frozen"] and c["has_dcnatten"] and c["has_scaleaggre"])
+        nf = c["num_frame"]
+        ok = (c["inch"] == 2 and c["basech"] == 8 and isinstance(nf, int) and nf >= 3 and nf % 2 == 1 and c["norm"] is None
+              and c["activation"] == "relu" and c["has_ltc"] and c["has_gtc"] and not c["gtc_frozen"] and c["has_dcnatten"]
+              and c["has_scaleaggre"])
         if not ok:
             raise _lib.ESRError("esr_b200.DeepRecurrNet: the sm_90a plan implements the shipped configuration "
-                                "(inch=2, basech=8, num_frame=3, norm=None, relu, all blocks on; "
-                                f"config/train_ours_enfssyn.yml:21-26); got {c}")
+                                "(inch=2, basech=8, norm=None, relu, all blocks on; config/train_ours_enfssyn.yml:21-26) "
+                                f"with an odd num_frame >= 3 (models/model.py:163-166); got {c}")
 
     def _packed_params(self, device):
         params = list(self.state_dict(keep_vars=True).values())
@@ -167,11 +169,12 @@ class DeepRecurrNet(nn.Module):
             tensors = [p.detach().to(device=device, dtype=torch.float32).contiguous() for p in params]
             arr = (ctypes.c_void_p * len(tensors))(*[t.data_ptr() for t in tensors])
             if self._blob is None or self._blob.device != device:
-                self._blob = torch.empty((L.esr_net_param_bytes(),), dtype=torch.uint8, device=device)
+                self._blob = torch.empty((L.esr_net_param_bytes_n(self._cfg["num_frame"]),), dtype=torch.uint8, device=device)
                 for p in self._plans.values():
                     p.close()
                 self._plans = {}
-            _lib.check(L.esr_net_pack_params(arr, _lib.ptr(self._blob), _lib.stream_ptr()), "esr_net_pack_params")
+            _lib.check(L.esr_net_pack_params_n(self._cfg["num_frame"], arr, _lib.ptr(self._blob), _lib.stream_ptr()),
+                       "esr_net_pack_params_n")
             torch.cuda.current_stream().synchronize()      # `tensors` may be temporaries
             self._blob_sig = sig
         return self._blob
@@ -234,10 +237,10 @@ class DeepRecurrNet(nn.Module):
         return out
 
     def forward_sequence(self, frames):
-        """frames: BxLx2xHxW (L >= num_frame) -> (L-2)*B x 2 x H x W, window-major (w*B + b): the L-2 sliding-window
-        forwards of the reference's loop (train_ours_cnt_seq.py:217-231) in ONE plan -- per-frame layers run once per
-        frame, state-independent layers once for all windows, only the ConvGRU chain is serial.  The carried state is
-        read at the start and left as after the last window, exactly as L-2 successive forward() calls would."""
+        """frames: BxLx2xHxW (L >= N = num_frame) -> (L-N+1)*B x 2 x H x W, window-major (w*B + b): the L-N+1
+        sliding-window forwards of the reference's loop (train_ours_cnt_seq.py:217-231) in ONE plan -- per-frame layers run
+        once per frame, state-independent layers once for all windows, only the ConvGRU chain is serial.  The carried state
+        is read at the start and left as after the last window, exactly as L-N+1 successive forward() calls would."""
         self._check_supported()
         if not frames.is_cuda:
             raise _lib.ESRError("esr_b200.DeepRecurrNet.forward_sequence needs a CUDA tensor (there is no CPU path)")

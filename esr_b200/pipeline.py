@@ -7,8 +7,8 @@ sliding windows) and the redistribution API (dataloader/cython_cnt2event/cnt2eve
 on the GPU and no intermediate host round trip:
 
     host events (pinned) --H2D--> esr_scatter_cnt (LR->HR lift fused) --> frame bank [B*L,2,kH,kW]
-        --> L-2 x esr_net_forward (windows addressed by index into the bank; ConvGRU state carried)
-        --> esr_expand_count / esr_expand_emit on all window outputs --> events [B*(L-2), maxlen, 4] --D2H--> host
+        --> L-N+1 x esr_net_forward (N = the model's num_frame; windows addressed by index into the bank; ConvGRU state carried)
+        --> esr_expand_count / esr_expand_emit on all window outputs --> events [B*(L-N+1), maxlen, 4] --D2H--> host
 """
 import torch
 
@@ -21,7 +21,10 @@ class EventSRPipeline:
         self.model, self.B, self.L, self.scale, self.dev = model, B, L, scale, device
         self.lr_size = (int(lr_size[0]), int(lr_size[1]))
         self.hr_size = (self.lr_size[0] * scale, self.lr_size[1] * scale)
-        N = 3
+        N = model._cfg["num_frame"]                  # frames per window (the config's SEQN)
+        if L < N:
+            raise ValueError(f"EventSRPipeline: L={L} frames per sequence is fewer than the model's num_frame={N}")
+        self.num_frame = N
         self.window_index = [
             torch.tensor([b * L + w + n for b in range(B) for n in range(N)], dtype=torch.int32, device=device)
             for w in range(L - N + 1)]
@@ -97,7 +100,7 @@ class EventSRPipeline:
 
     @torch.no_grad()
     def run_device(self, xs, ys, ps, frame_off, n_max_frame, mode=0):
-        """All inputs already on the GPU.  Returns (sr_cnt [B*(L-2),2,kH,kW], events [B*(L-2),maxlen,4]) on the GPU.
+        """All inputs already on the GPU.  Returns (sr_cnt [B*(L-N+1),2,kH,kW], events [B*(L-N+1),maxlen,4]) on the GPU.
         Sample order of the outputs: window-major (w * B + b).  With captured graphs both tensors are views of the graph's static
         buffers: valid until the next call."""
         encodings.encode_frames(xs, ys, ps, frame_off, lr_size=self.lr_size, hr_size=self.hr_size,

@@ -1,6 +1,6 @@
 """Training step of the hot path (SURVEY.md 8a row 17; train_ours_cnt_seq.py:206-235, 767-782).
 
-The reference sums MSELoss(pred, gt) over the L-2 windows of a sequence (ConvGRU state carried, so gradients flow back
+The reference sums MSELoss(pred, gt) over the L-N+1 windows of a sequence (ConvGRU state carried, so gradients flow back
 through time across windows), calls backward once, lets DDP all-reduce the 1 813 120 gradients and steps
 Adam(lr, weight_decay, amsgrad).  Here
 
@@ -263,16 +263,16 @@ def _accumulate(param, grad):
 
 
 def forward_sequence(model, frames, states=None):
-    """frames BxLx2xHxW (L >= num_frame) -> ((L-2)*B x 2 x H x W window-major, [h_fwd, h_rev]).
+    """frames BxLx2xHxW (L >= N = num_frame) -> ((L-N+1)*B x 2 x H x W window-major, [h_fwd, h_rev]).
 
-    The L-2 sliding-window forwards of the reference's training loop (train_ours_cnt_seq.py:217-231) as ONE differentiable
+    The L-N+1 sliding-window forwards of the reference's training loop (train_ours_cnt_seq.py:217-231) as ONE differentiable
     graph with the same batching as the inference plan (DESIGN.md 5): head / encoder / attention maps once per frame,
     every state-independent layer once for all windows, only the ConvGRU chain serial (both directions batched as 2B).
     Per image the arithmetic is that of models/model.py:314-344; gradients w.r.t. parameters, frames and `states`."""
     cfg = model._cfg
     N = cfg["num_frame"]
     B, L, Cin, H, W = frames.shape
-    assert L >= N and N == 3
+    assert L >= N
     Wn = L - N + 1
     Hc, Wc = 8 * math.ceil(H / 8), 8 * math.ceil(W / 8)
     x = frames.float().transpose(0, 1).reshape(L * B, Cin, H, W)          # frame-major: image l*B + b
@@ -291,7 +291,8 @@ def forward_sequence(model, frames, states=None):
     #                                                                       (indexing would zero-fill a full tensor per use)
     # ---- TimePropagation.local_time_corre (models/model.py:77-89, 133-146) for every (window, slot)
     tp = model.time_propagate
-    pairs = sorted({(j, j) for j in range(Wn)} | {(j + 2, j + 2) for j in range(Wn)} | {(j, j + 1) for j in range(L - 1)})
+    # the (frame, frame) pairs the LTC index rule touches: (w, w) and (w+N-1, w+N-1) at a window's edges, neighbours inside
+    pairs = sorted({(j, j) for j in range(Wn)} | {(j + N - 1, j + N - 1) for j in range(Wn)} | {(j, j + 1) for j in range(L - 1)})
     pm_in = torch.cat([torch.cat([f[a], f[b]], 1) for a, b in pairs], 0)
     pm = _cl(tp.pred_map[1], _cl(tp.pred_map[0], pm_in, act="relu"), act="sigmoid").view(len(pairs), B, 1, h, w).unbind(0)
     gate = {p: pm[k] for k, p in enumerate(pairs)}
@@ -300,7 +301,7 @@ def forward_sequence(model, frames, states=None):
         for i in range(N):
             a, b, c = wi + max(i - 1, 0), wi + i, wi + min(i + 1, N - 1)
             cat_in.append(torch.cat([f[a] * gate[(a, b)], f[b], f[c] * gate[(b, c)]], 1))
-    xcat = torch.cat(cat_in, 0)                                           # [(Wn*3*B), 192, h, w]
+    xcat = torch.cat(cat_in, 0)                                           # [(Wn*N*B), 192, h, w]
     rb = tp.local_fusion[0]                                               # ResidualBlock (models/submodules.py:391-409)
     r = conv2d(xcat, rb.conv1.weight, rb.conv1.bias, 1, "relu")
     r = torch.relu(conv2d(r, rb.conv2.weight, rb.conv2.bias, 1, None) + xcat)
@@ -341,7 +342,7 @@ def forward_sequence(model, frames, states=None):
             rev_w[N - 1 - i] = hr
         rev.extend(rev_w)
     new_states = [None, None] if cfg["gtc_frozen"] else list(hs.split(B, 0))
-    both = torch.cat([torch.cat(fwd, 0), torch.cat(rev, 0)], 1)           # [(Wn*3*B), 128, h, w]
+    both = torch.cat([torch.cat(fwd, 0), torch.cat(rev, 0)], 1)           # [(Wn*N*B), 128, h, w]
     prop = (_cl(tp.global_fusion, both, act="relu") + mid_feat).view(Wn, N, B, C, h, w).unbind(1)
 
     # ---- STFusion (models/model.py:208-291): both neighbours of all windows at once
@@ -368,7 +369,7 @@ def forward_sequence(model, frames, states=None):
     x = _cl(sf.dense_fusion[1], _cl(sf.dense_fusion[0], x, act="relu"))
     for lvl, ft in enumerate(pyramid):                                    # scale_aggre + recons (models/model.py:253-291)
         prod = (ft * _cl(sf.attens[lvl], ft, act="sigmoid")).view(L, B, *ft.shape[1:]).unbind(0)
-        agg = torch.cat([(prod[wi] + prod[wi + 1] + prod[wi + 2]) / N for wi in range(Wn)], 0)
+        agg = torch.cat([_window_sum(prod, wi, N) / N for wi in range(Wn)], 0)   # mean over the window's N frames
         x = upsample2x(x + agg)
         x = _cl(sf.recons[lvl], x, act="relu")
     x = _cl(model.tail, x, act="relu")
@@ -376,6 +377,14 @@ def forward_sequence(model, frames, states=None):
         cy, cx = Hc // 2, Wc // 2
         x = x[..., cy - H // 2: cy + math.ceil(H / 2), cx - W // 2: cx + math.ceil(W / 2)].contiguous()
     return x, new_states
+
+
+def _window_sum(prod, wi, N):
+    """prod[wi] + prod[wi + 1] + ... + prod[wi + N - 1], added in frame order."""
+    s = prod[wi]
+    for i in range(1, N):
+        s = s + prod[wi + i]
+    return s
 
 
 def forward_window(model, inp, states=None):
@@ -504,24 +513,35 @@ def _step_body(model, optimizer, frames, gt, num_frame, all_reduce):
     return loss.detach()
 
 
-def train_step(model, optimizer, frames, gt, num_frame=3, all_reduce=None):
+def _model_num_frame(model, num_frame):
+    """The model's num_frame (model._cfg, or model.module._cfg under DDP); an explicit value must agree with it."""
+    net = model.module if hasattr(model, "module") else model
+    n = net._cfg["num_frame"]
+    if num_frame is not None and int(num_frame) != n:
+        raise _lib.ESRError(f"esr_b200.train: num_frame={num_frame} but the model was built with num_frame={n}")
+    return n
+
+
+def train_step(model, optimizer, frames, gt, num_frame=None, all_reduce=None):
     """One reference training iteration (train_ours_cnt_seq.py:209-235) on a batch of sequences.
 
     frames: BxLx2xHxW input count tensors (inp_scaled_cnt of each frame); gt: BxLx2xHxW target count tensors.
-    Windows slide by one frame (dataloader/h5dataloader.py:229-231); the loss is the sum over windows of
+    Windows of num_frame frames (default and required: the model's) slide by one frame (dataloader/h5dataloader.py:229-231);
+    the loss is the sum over windows of
     MSE(pred, gt[:, window middle]) with the ConvGRU state carried from window to window; one backward; optional
     `all_reduce(exchange)` over the flat gradient bucket + the two logging scalars (DDP's role when the model is not
     DDP-wrapped; after it `optimizer.log` holds the rank-reduced last-window MSE and summed loss, which is everything
     train_ours_cnt_seq.py:238-239 + :339 need -- no extra barrier or collective); one Adam step.  Returns the local summed loss."""
-    return _step_body(model, optimizer, frames, gt, num_frame, all_reduce)
+    return _step_body(model, optimizer, frames, gt, _model_num_frame(model, num_frame), all_reduce)
 
 
 class GraphedTrainStep:
     """train_step captured once into a CUDA graph (forward, backward, all-reduce hook and the Adam kernel) and replayed:
     no Python / launch overhead per iteration.  Shapes are fixed at construction; data is copied into static buffers."""
 
-    def __init__(self, model, optimizer, frames_shape, device, num_frame=3, all_reduce=None, warmup=2):
+    def __init__(self, model, optimizer, frames_shape, device, num_frame=None, all_reduce=None, warmup=2):
         self.model, self.opt = model, optimizer
+        num_frame = _model_num_frame(model, num_frame)
         self.frames = torch.zeros(frames_shape, dtype=torch.float32, device=device)
         self.gt = torch.zeros(frames_shape, dtype=torch.float32, device=device)
         keep = [t.clone() for t in (optimizer.flat, optimizer.exp_avg, optimizer.exp_avg_sq)]

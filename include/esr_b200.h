@@ -150,6 +150,11 @@ typedef struct esr_conv_desc {
 } esr_conv_desc;
 
 int esr_conv_tc(const esr_conv_desc *desc, esr_stream_t stream);
+/* Same, with sources that repeat over images: for each s < n_src, chunk_img_step[s] = k != 0 makes source s (64 channels)
+ * contribute src_chunks[s] 64-channel chunks, chunk j read from image src_img[s][img] + j*k (identity map: img + j*k).
+ * This is the channel concatenation of images of one tensor (dense_fusion.0 over the num_frame-1 aligned neighbours).
+ * Host arrays of 3 ints; NULL = all zero (then the call is esr_conv_tc). */
+int esr_conv_tc_chunked(const esr_conv_desc *desc, const int *src_chunks, const int *chunk_img_step, esr_stream_t stream);
 size_t esr_conv_weight_bytes(int cout, int cin, int ksz);
 /* w1 != NULL: two [cout_each,cin,k,k] tensors concatenated along Cout (GRU update|reset) */
 int esr_pack_conv_weight(const float *w0, const float *w1, int cout_each, int cin, int ksz, void *dst,
@@ -163,14 +168,21 @@ int esr_split_to_nchw(const void *src, int n_img, int C, int H, int W, float *ds
  * models/model.py:20-291, models/submodules.py (ConvLayer, UpsampleConvLayer, ResidualBlock, RecurrentConvLayer,
  * ConvGRU, MLP), models/model_util.py:133-164 (CropSize) and the `_ext.dcn_v2_forward` operator
  * (models/DCNv2/src/dcn_v2.h:9-27, src/cuda/dcn_v2_cuda.cu:20-95) for the shipped configuration
- * (inch=2, basech=8, num_frame=3, norm=None, relu, all sub-blocks enabled; config/train_ours_enfssyn.yml:21-26).
+ * (inch=2, basech=8, norm=None, relu, all sub-blocks enabled; config/train_ours_enfssyn.yml:21-26) and any odd
+ * num_frame N >= 3 (the config's SEQN; the shipped value is 3).
  *
  *  params    : 68 device pointers to fp32 tensors in the reference's state_dict order
  *              (head.conv2d.weight, head.conv2d.bias, feat_extract.convblock.0.conv2d.weight, ... tail.conv2d.bias)
- *  blob      : esr_net_param_bytes() bytes; repack whenever the parameters change
+ *  blob      : esr_net_param_bytes_n(N) bytes, packed by esr_net_pack_params_n(N, ...) for the N the net is created with;
+ *              repack whenever the parameters change.  Only dense_fusion.0's weight (N*64 input channels) depends on N,
+ *              so a blob packed for another N has a different layout: esr_net_create refuses one that is too short for N
+ *              when the device allocation holding it says so, and cannot detect the other mismatches.
+ *              esr_net_param_bytes() / esr_net_pack_params() are the N = 3 forms.
  *  workspace : esr_net_workspace_bytes(B,N,L,H,W) bytes, owned by the caller, must outlive the net; holds all
  *              intermediates AND the recurrent states (which persist across esr_net_forward calls)
- *  L         : frames per sequence handled by one call.  L == N (=3) is the reference's forward: one window,
+ *  N         : num_frame, odd and >= 3 (anything else: ESR_EUNSUPPORTED).  The middle frame (N-1)/2 of each window is
+ *              the one super-resolved.
+ *  L         : frames per sequence handled by one call.  L == N is the reference's forward: one window,
  *              input fp32 [B,N,2,H,W], output fp32 [B,2,H,W].  L > N is the sequence form used by the pipeline:
  *              input fp32 [B,L,2,H,W], output fp32 [(L-N+1)*B,2,H,W] (window-major: w*B+b) = the L-N+1 sliding-window
  *              forwards the reference would run one after another with the state carried (train_ours_cnt_seq.py:217-231,
@@ -181,8 +193,10 @@ int esr_split_to_nchw(const void *src, int n_img, int C, int H, int W, float *ds
  * H, W need not be multiples of 8: the CropSize pad / crop is folded into the first and last kernels.
  * --------------------------------------------------------------------------------------------- */
 typedef void *esr_net_t;
-size_t esr_net_param_bytes(void);
+size_t esr_net_param_bytes(void);                 /* num_frame = 3 */
 int esr_net_pack_params(const float *const *params_host_array_of_device_ptrs, void *blob, esr_stream_t stream);
+size_t esr_net_param_bytes_n(int num_frame);      /* 0 for an unsupported num_frame */
+int esr_net_pack_params_n(int num_frame, const float *const *params_host_array_of_device_ptrs, void *blob, esr_stream_t stream);
 size_t esr_net_workspace_bytes(int B, int N, int L, int H, int W);
 int esr_net_create(esr_net_t *net, int B, int N, int L, int H, int W, void *blob, void *workspace, size_t workspace_bytes,
                    esr_stream_t stream);
