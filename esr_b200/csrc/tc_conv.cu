@@ -2,10 +2,10 @@
 //
 //   D[128 pixels, Cout] += A[128 pixels, 64 ch of one tap] * B[Cout, 64]^T      per K-block (tap x 64-channel chunk)
 //
-// * Activations live in HBM as "split bf16" NHWC tensors (value = hi + lo).  A K-block's A tile is ONE TMA box
-//   (64 ch, TW, TH, 1 image, 1 plane) taken at the tap's (dy, dx) shift; out-of-image coordinates are zero-filled
-//   by TMA, which is exactly the conv's zero padding.  The box lands in shared memory in the 128B-swizzled K-major
-//   layout that wgmma reads, so no thread touches the operands.
+// * Activations live in HBM as "split bf16" NHWC tensors (value = hi + lo).  A 3x3 layer's A operand is ONE TMA box
+//   (64 ch, TW, TH + 2, 1 image, 1 plane) per 64-channel chunk and dx shift, read by the three dy taps at row offsets
+//   0, TW, 2 TW; out-of-image coordinates are zero-filled by TMA, which is exactly the conv's zero padding.  The box lands
+//   in shared memory in the 128B-swizzled K-major layout that wgmma reads, so no thread touches the operands.
 // * Channel concatenation (torch.cat in the reference) is a K-split over up to 3 source tensors.  A 64-channel source can also
 //   stand for several chunks, chunk j at image + j * step (the num_frame-way concatenation of dense_fusion): one multiply-add
 //   in the producer per K-block.
@@ -14,7 +14,8 @@
 // * Warp roles: warps 0-7 = two consumer warpgroups (pixel rows 0-63 / 64-127 of the tile, accumulators in registers,
 //   then the epilogue: staging through shared memory -> bias / residual / activation / GRU gating -> split-bf16 or fp32
 //   stores); warp 8 = TMA producer.
-// * mbarrier ring: full[s] (TMA -> consumers), empty[s] (one arrival per consumer warp once its MMAs on s retired -> TMA).
+// * Two mbarrier rings, A boxes and per-tap weights: full[s] (TMA -> consumers), empty[s] (one arrival per consumer warp
+//   once its MMAs on s retired -> TMA).
 //
 // Reference layers served: every Conv2d of models/model.py at feature resolution (Cin multiple of 64), the ConvGRU
 // gates (models/submodules.py:496-514) and the DCNv2 contraction (models/DCNv2/src/cuda/dcn_v2_cuda.cu:90-92).
@@ -28,41 +29,74 @@ constexpr int TC_THREADS = 288;
 
 // ------------------------------------------------------------------------------------------------
 // Persistent conv body: the CTA walks tiles tile0, tile0 + step, ... of one layer (128 output pixels (TH x TW) of one image x
-// all NP (= npad) output channels each).  The TMA producer streams K-blocks across tile boundaries through the ring, so the
-// loads of tile i+1 overlap the epilogue of tile i; the ring position (s, ph) of each role persists across tiles and calls.
-// The epilogue stages accumulators in a dedicated area beside the ring (the ring is already refilling).
+// all NP (= npad) output channels each).  K-blocks run in the order (chunk, dx, dy).  A 3x3 layer loads ONE A box of
+// TW x (TH + 2) pixels per (chunk, dx), taken at (x0 + dx, y0 - 1); its three dy taps are the 128 rows starting (dy + 1) TW
+// rows into it (a multiple of 1024 bytes, so every tap starts on a SWIZZLE_128B atom).  A 1x1 layer loads the tile itself, one
+// tap per box.  A boxes and per-tap weights (B) have separate rings: a consumer frees an A box once the MMAs of its last tap
+// retired, and each B slot once its own MMAs did.  The TMA producer streams both across tile boundaries, so the loads of
+// tile i+1 overlap the epilogue of tile i; the ring positions of each role persist across tiles and calls.
+// The epilogue stages accumulators in a dedicated area beside the rings (the rings are already refilling).
 // ------------------------------------------------------------------------------------------------
 struct TcSmem {
-    uint32_t ring, stage_stride, bar_full, bar_empty;   // shared-memory addresses
-    float *stg;                                         // epilogue staging: [2 warpgroups][64][TC_STG_LD] fp32
-    int stages;
+    uint32_t a_ring, a_box, b_ring, b_slot;              // shared-memory addresses and slot strides
+    uint32_t bar;                                        // mbarriers: A full [na], A empty [na], B full [nb], B empty [nb]
+    float *stg;                                          // epilogue staging: [2 warpgroups][64][TC_STG_LD] fp32
+    int na, nb;
+    __device__ uint32_t a_full(uint32_t s) const { return bar + 8u * s; }
+    __device__ uint32_t a_empty(uint32_t s) const { return bar + 8u * (na + s); }
+    __device__ uint32_t b_full(uint32_t s) const { return bar + 8u * (2 * na + s); }
+    __device__ uint32_t b_empty(uint32_t s) const { return bar + 8u * (2 * na + nb + s); }
 };
-struct TcRing { uint32_t s = 0, ph = 0; };
+// Ring position: the count of slots used modulo twice the depth n, i.e. slot c % n with phase c / n (one register per ring).
+struct TcRing { uint32_t ca = 0, cb = 0; };
+__device__ __forceinline__ uint32_t ring_slot(uint32_t c, int n) { return c < (uint32_t)n ? c : c - n; }
+__device__ __forceinline__ uint32_t ring_phase(uint32_t c, int n) { return c < (uint32_t)n ? 0u : 1u; }
+__device__ __forceinline__ uint32_t ring_next(uint32_t c, int n) { return c + 1 == 2u * n ? 0u : c + 1; }
+__device__ __forceinline__ uint32_t ring_prev_slot(uint32_t c, int n) { return ring_slot(c == 0 ? 2u * n - 1 : c - 1, n); }
 
-// 1024: worst-case alignment of the ring; then the ring, the two staging tiles and the full / empty mbarriers.  npad = 256 at
-// the minimum of two stages takes exactly the 227 KB (232448 B) an H100 block may opt in to: nothing more fits beside it
-// (conv_tc_prepare refuses a width that does not fit instead of failing at launch).
-static size_t tc_smem_bytes(int npad, int stages)
+// 1024: worst-case alignment of the rings; then the A ring, the B ring, the two staging tiles and the full / empty mbarriers of
+// both rings.  conv_tc_prepare and gru_chain_prepare size the rings so that this fits the 227 KB (232448 B) an H100 block
+// may opt in to.
+static size_t tc_smem_bytes(int npad, uint32_t a_box, int na, int nb)
 {
-    return 1024 + (size_t)stages * (2 * TC_A_BYTES + 2 * (size_t)npad * 128) + 2 * TC_STG_BYTES + 16 * (size_t)stages;
+    return 1024 + (size_t)na * (a_box + 16) + (size_t)nb * (2 * (size_t)npad * 128 + 16) + 2 * TC_STG_BYTES;
 }
-__device__ __forceinline__ TcSmem tc_smem_layout(int np_max, int stages)
+// Ring depths for one CTA per SM: two A boxes and two B slots (one A box where that does not fit: npad = 256), then one more slot
+// for whichever ring is fewer K-blocks ahead (B on a tie) while it fits, up to 4 A boxes and 9 B slots.  false: nothing fits.
+static bool tc_rings(int npad, uint32_t a_box, int taps, size_t cap, int *na_out, int *nb_out)
+{
+    int na = 2, nb = 2;
+    if (tc_smem_bytes(npad, a_box, na, nb) > cap) na = 1;
+    if (tc_smem_bytes(npad, a_box, na, nb) > cap) return false;
+    for (;;) {
+        const bool a_can = na < 4 && tc_smem_bytes(npad, a_box, na + 1, nb) <= cap;
+        const bool b_can = nb < 9 && tc_smem_bytes(npad, a_box, na, nb + 1) <= cap;
+        if (a_can && (!b_can || (na - 1) * taps < nb - 1)) ++na;
+        else if (b_can) ++nb;
+        else break;
+    }
+    *na_out = na; *nb_out = nb;
+    return true;
+}
+__device__ __forceinline__ TcSmem tc_smem_layout(int np_max, uint32_t a_box, int na, int nb)
 {
     extern __shared__ uint8_t smem_raw[];
     TcSmem m;
-    m.ring = (smem_u32(smem_raw) + 1023u) & ~1023u;                    // SWIZZLE_128B needs 1024-B alignment
-    m.stage_stride = 2u * TC_A_BYTES + 2u * (uint32_t)np_max * 128u;
-    const uint32_t stg = m.ring + (uint32_t)stages * m.stage_stride;
+    m.a_ring = (smem_u32(smem_raw) + 1023u) & ~1023u;                  // SWIZZLE_128B needs 1024-B alignment
+    m.a_box = a_box;                                                    // a multiple of 1024 (TW is)
+    m.b_ring = m.a_ring + (uint32_t)na * a_box;
+    m.b_slot = 2u * (uint32_t)np_max * 128u;
+    const uint32_t stg = m.b_ring + (uint32_t)nb * m.b_slot;
     m.stg = reinterpret_cast<float *>(smem_raw + (stg - smem_u32(smem_raw)));
-    m.bar_full = stg + 2u * TC_STG_BYTES;
-    m.bar_empty = m.bar_full + 8u * stages;
-    m.stages = stages;
+    m.bar = stg + 2u * TC_STG_BYTES;
+    m.na = na; m.nb = nb;
     return m;
 }
 __device__ __forceinline__ void tc_init_barriers(const TcSmem &m)
 {
     if (threadIdx.x == 0) {
-        for (int s = 0; s < m.stages; ++s) { mbar_init(m.bar_full + 8u * s, 1); mbar_init(m.bar_empty + 8u * s, 8); }
+        for (int s = 0; s < m.na; ++s) { mbar_init(m.a_full(s), 1); mbar_init(m.a_empty(s), 8); }
+        for (int s = 0; s < m.nb; ++s) { mbar_init(m.b_full(s), 1); mbar_init(m.b_empty(s), 8); }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
     __syncthreads();
@@ -71,37 +105,47 @@ __device__ __forceinline__ void tc_init_barriers(const TcSmem &m)
 template <int NP>
 __device__ __forceinline__ void conv_tiles(const ConvTCArgs &a, int tile0, int step, const TcSmem &m, TcRing &ring)
 {
-    constexpr uint32_t b_bytes = (uint32_t)NP * 128u;
-    constexpr uint32_t tx_bytes = 2u * TC_A_BYTES + 2u * b_bytes;
+    constexpr uint32_t b_bytes = (uint32_t)NP * 128u;                  // one plane of one tap's weights
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int tiles_per_img = a.tiles_x * a.tiles_y, n_tiles = a.n_img * tiles_per_img;
+    const bool k3 = a.ntaps == 9;
+    const int taps = k3 ? 3 : 1, nbox = a.nkb / taps;                  // dy taps per A box, A boxes per tile
+    const uint32_t a_plane = m.a_box / 2;
 
     if (warp == 8) {
         // ===================== TMA producer (one elected lane; the others idle until the caller's next barrier) =====================
         if (elect_one_sync()) {
-            uint32_t s = ring.s, ph = ring.ph;
+            uint32_t ca = ring.ca, cb = ring.cb;
             for (int tile = tile0; tile < n_tiles; tile += step) {
                 const int img = tile / tiles_per_img, trem = tile - img * tiles_per_img;
                 const int y0 = (trem / a.tiles_x) * a.TH, x0 = (trem % a.tiles_x) * a.TW;
                 int src = 0, chunk_base = 0;
-                for (int kb = 0; kb < a.nkb; ++kb) {
-                    const int gchunk = kb / a.ntaps, tap = kb - gchunk * a.ntaps;
+                for (int bx = 0; bx < nbox; ++bx) {
+                    const int gchunk = k3 ? bx / 3 : bx, dx = k3 ? bx - 3 * gchunk - 1 : 0;
                     while (gchunk >= a.chunk_end[src]) { chunk_base = a.chunk_end[src]; ++src; }
-                    const int dy = a.ntaps == 9 ? tap / 3 - 1 : 0, dx = a.ntaps == 9 ? tap % 3 - 1 : 0;
                     const int cc = gchunk - chunk_base, istep = a.chunk_img_step[src];
                     const int simg = (a.src_img[src] ? a.src_img[src][img] : img) + cc * istep;
-                    mbar_wait(m.bar_empty + 8u * s, ph ^ 1u);
-                    mbar_expect_tx(m.bar_full + 8u * s, tx_bytes);
-                    const uint32_t st = m.ring + s * m.stage_stride;
                     const int c0 = istep ? 0 : cc * 64;
-                    tma_load_5d(&a.amap[src], m.bar_full + 8u * s, st, c0, x0 + dx, y0 + dy, simg, 0);
-                    tma_load_5d(&a.amap[src], m.bar_full + 8u * s, st + TC_A_BYTES, c0, x0 + dx, y0 + dy, simg, 1);
-                    tma_load_3d(&a.bmap, m.bar_full + 8u * s, st + 2u * TC_A_BYTES, 0, 0, kb);
-                    tma_load_3d(&a.bmap, m.bar_full + 8u * s, st + 2u * TC_A_BYTES + b_bytes, 0, 0, a.nkb + kb);
-                    if (++s == (uint32_t)m.stages) { s = 0; ph ^= 1u; }
+                    const uint32_t sa = ring_slot(ca, m.na);
+                    mbar_wait(m.a_empty(sa), ring_phase(ca, m.na) ^ 1u);
+                    mbar_expect_tx(m.a_full(sa), m.a_box);
+                    const uint32_t as = m.a_ring + sa * m.a_box;
+                    tma_load_5d(&a.amap[src], m.a_full(sa), as, c0, x0 + dx, y0 - (k3 ? 1 : 0), simg, 0);
+                    tma_load_5d(&a.amap[src], m.a_full(sa), as + a_plane, c0, x0 + dx, y0 - (k3 ? 1 : 0), simg, 1);
+                    ca = ring_next(ca, m.na);
+                    for (int t = 0; t < taps; ++t) {
+                        const int kb = k3 ? gchunk * 9 + 3 * t + dx + 1 : gchunk;   // the packing's order: chunk * 9 + 3 (dy + 1) + dx + 1
+                        const uint32_t sb = ring_slot(cb, m.nb);
+                        mbar_wait(m.b_empty(sb), ring_phase(cb, m.nb) ^ 1u);
+                        mbar_expect_tx(m.b_full(sb), 2u * b_bytes);
+                        const uint32_t bs = m.b_ring + sb * m.b_slot;
+                        tma_load_3d(&a.bmap, m.b_full(sb), bs, 0, 0, kb);
+                        tma_load_3d(&a.bmap, m.b_full(sb), bs + b_bytes, 0, 0, a.nkb + kb);
+                        cb = ring_next(cb, m.nb);
+                    }
                 }
             }
-            ring.s = s; ring.ph = ph;
+            ring.ca = ca; ring.cb = cb;
         }
         return;
     }
@@ -110,19 +154,22 @@ __device__ __forceinline__ void conv_tiles(const ConvTCArgs &a, int tile0, int s
     const int wg = warp >> 2;
     float *stg = m.stg + wg * (TC_STG_BYTES / 4);
     const int r = threadIdx.x & 63, h = (threadIdx.x >> 6) & 1;
-    uint32_t s = ring.s, ph = ring.ph;
+    const uint32_t tap_rows = (uint32_t)a.TW * 128u;                   // bytes between the dy taps of a box
+    uint32_t ca = ring.ca, cb = ring.cb;
     for (int tile = tile0; tile < n_tiles; tile += step) {
         const int img = tile / tiles_per_img, trem = tile - img * tiles_per_img;
         const int y0 = (trem / a.tiles_x) * a.TH, x0 = (trem % a.tiles_x) * a.TW;
         float acc[NP / 2];
 #pragma unroll
         for (int i = 0; i < NP / 2; ++i) acc[i] = 0.0f;
-        uint32_t prev = 0;
-        for (int kb = 0; kb < a.nkb; ++kb) {
-            mbar_wait(m.bar_full + 8u * s, ph);
-            const uint32_t st = m.ring + s * m.stage_stride;
-            const uint64_t dah = wgmma_desc(st + (uint32_t)wg * 8192u), dal = wgmma_desc(st + TC_A_BYTES + (uint32_t)wg * 8192u);
-            const uint64_t dbh = wgmma_desc(st + 2u * TC_A_BYTES), dbl = wgmma_desc(st + 2u * TC_A_BYTES + b_bytes);
+        for (int kb = 0, t = 0; kb < a.nkb; ++kb) {                    // t: the K-block's tap within its A box
+            const uint32_t sa = ring_slot(ca, m.na), sb = ring_slot(cb, m.nb);
+            if (t == 0) mbar_wait(m.a_full(sa), ring_phase(ca, m.na));
+            mbar_wait(m.b_full(sb), ring_phase(cb, m.nb));
+            const uint32_t ah = m.a_ring + sa * m.a_box + (uint32_t)wg * 8192u + (uint32_t)t * tap_rows;
+            const uint32_t bs = m.b_ring + sb * m.b_slot;
+            const uint64_t dah = wgmma_desc(ah), dal = wgmma_desc(ah + a_plane);
+            const uint64_t dbh = wgmma_desc(bs), dbl = wgmma_desc(bs + b_bytes);
             acc_fence<NP / 2>(acc);
             wgmma_fence();
 #pragma unroll
@@ -132,15 +179,26 @@ __device__ __forceinline__ void conv_tiles(const ConvTCArgs &a, int tile0, int s
                 wgmma_rows<NP, 0>(acc, dah + 2 * k, dbh + 2 * k);
             }
             wgmma_commit();
-            wgmma_wait<1>();                                        // the previous K-block's MMAs have retired: free its stage
+            // the previous K-block's MMAs have retired: free its B slot, and at a box's first tap the previous box.  With a
+            // single A box (npad >= 224) the box's last tap waits for its own MMAs and frees it at once: the next box needs it.
+            const bool drain = m.na == 1 && t == taps - 1;
+            if (drain) wgmma_wait<0>();
+            else wgmma_wait<1>();
             acc_fence<NP / 2>(acc);
-            if (kb > 0 && lane == 0) mbar_arrive(m.bar_empty + 8u * prev);
-            prev = s;
-            if (++s == (uint32_t)m.stages) { s = 0; ph ^= 1u; }
+            if (lane == 0) {
+                if (kb != 0) mbar_arrive(m.b_empty(ring_prev_slot(cb, m.nb)));
+                if (kb != 0 && t == 0 && m.na > 1) mbar_arrive(m.a_empty(ring_prev_slot(ca, m.na)));
+                if (drain) mbar_arrive(m.a_empty(0));                 // the only slot
+            }
+            cb = ring_next(cb, m.nb);
+            if (++t == taps) { t = 0; ca = ring_next(ca, m.na); }
         }
         wgmma_wait<0>();
         acc_fence<NP / 2>(acc);
-        if (lane == 0) mbar_arrive(m.bar_empty + 8u * prev);      // the tile's last stage
+        if (lane == 0) {                                            // the tile's last K-block and box
+            mbar_arrive(m.b_empty(ring_prev_slot(cb, m.nb)));
+            if (m.na > 1) mbar_arrive(m.a_empty(ring_prev_slot(ca, m.na)));
+        }
 
         // ===================== epilogue: thread = (tile row r, 32-column half h) per 64-column pass =====================
         const int mrow = wg * 64 + r;                               // accumulator row = pixel within the tile
@@ -160,15 +218,15 @@ __device__ __forceinline__ void conv_tiles(const ConvTCArgs &a, int tile0, int s
             named_sync(2 + wg, 128);
         }
     }
-    ring.s = s; ring.ph = ph;
+    ring.ca = ca; ring.cb = cb;
 }
 
 // one layer: grid = min(tiles, resident CTAs); CTA b takes tiles b, b + gridDim.x, ...
 template <int NP>
-__global__ void __launch_bounds__(TC_THREADS, NP <= 64 ? 2 : 1) k_conv_tc(const __grid_constant__ ConvTCArgs a)
+__global__ void __launch_bounds__(TC_THREADS, 1) k_conv_tc(const __grid_constant__ ConvTCArgs a)
 {
     PDL_LAUNCH_DEPENDENTS();
-    const TcSmem m = tc_smem_layout(NP, a.stages);
+    const TcSmem m = tc_smem_layout(NP, tc_a_box_bytes(a.TW, a.TH, a.ntaps), a.a_stages, a.b_stages);
     tc_init_barriers(m);
     PDL_WAIT();                      // everything above is CTA-local set-up; global memory only from here on
     TcRing ring;
@@ -198,10 +256,10 @@ __device__ __forceinline__ void grid_barrier(unsigned int *ctr, unsigned int tar
     asm volatile("fence.proxy.async.global;" ::: "memory");
 }
 
-__global__ void __launch_bounds__(TC_THREADS, 1) k_gru_chain(const ConvTCArgs *__restrict__ args, int nphase, int stages,
+__global__ void __launch_bounds__(TC_THREADS, 1) k_gru_chain(const ConvTCArgs *__restrict__ args, int nphase, int na, int nb,
                                                              unsigned int *ctr)
 {
-    const TcSmem m = tc_smem_layout(128, stages);
+    const TcSmem m = tc_smem_layout(128, tc_a_box_bytes(args[0].TW, args[0].TH, args[0].ntaps), na, nb);
     tc_init_barriers(m);
     TcRing ring;
     for (int p = 0; p < nphase; ++p) {
@@ -272,8 +330,9 @@ int conv_tc_prepare(const ConvTCDesc &d, ConvTCArgs *args)
     ESR_REQUIRE(d.ntaps == 9 || d.ntaps == 1, "conv_tc: ntaps=%d", d.ntaps);
     const int H = d.src[0].H, W = d.src[0].W;
     int chunks = 0;
-    // tile shape: 128 pixels; prefer wide tiles, but do not waste more than half a tile on narrow images
-    const int TW = W >= 24 ? 32 : (W >= 12 ? 16 : 8);
+    // tile shape: 128 pixels, 16 x 8 (8 x 16 on images narrower than 12, so that at most half a tile is wasted).  A 3x3 box of
+    // 16 x 10 pixels serves three taps: 2.4x fewer A bytes per tap than one box per tap (32 x 4 tiles: 2.0x).
+    const int TW = W >= 12 ? 16 : 8;
     const int TH = TC_BLOCK_M / TW;
     for (int s = 0; s < d.n_src; ++s) {
         const SplitTensor &t = d.src[s];
@@ -289,7 +348,7 @@ int conv_tc_prepare(const ConvTCDesc &d, ConvTCArgs *args)
         a.chunk_end[s] = chunks;
         a.chunk_img_step[s] = d.chunk_img_step[s];
         a.src_img[s] = d.src_img[s];
-        int rc = make_amap(t, TW, TH, &a.amap[s]);
+        int rc = make_amap(t, TW, tc_box_h(TH, d.ntaps), &a.amap[s]);
         if (rc) return rc;
     }
     for (int s = d.n_src; s < TC_MAX_SRC; ++s) a.chunk_end[s] = 1 << 30;
@@ -300,21 +359,12 @@ int conv_tc_prepare(const ConvTCDesc &d, ConvTCArgs *args)
     if (rc) return rc;
     a.H = H; a.W = W; a.TW = TW; a.TH = TH;
     a.tiles_x = (W + TW - 1) / TW; a.tiles_y = (H + TH - 1) / TH; a.n_img = d.n_img;
-    // Pipeline depth: all the stages that fit.  Grids of more than one wave keep two persistent CTAs resident per SM where the
-    // registers allow it (npad <= 64, see the kernel's launch bounds) and each fits in half the shared memory.
+    // Ring depths: as many slots as fit beside one CTA per SM (two 40 KB A boxes already rule out a second CTA).
     const size_t smem_cap = (size_t)dev_info().max_smem_optin;
-    const int n_tiles = d.n_img * a.tiles_x * a.tiles_y;
-    int stages = 6;
-    while (stages > 2 && tc_smem_bytes(a.npad, stages) > smem_cap) --stages;
-    if (n_tiles > dev_info().sm_count && a.npad <= 64) {
-        int s2 = stages;
-        while (s2 > 2 && 2 * (tc_smem_bytes(a.npad, s2) + 1024) > smem_cap) --s2;
-        if (2 * (tc_smem_bytes(a.npad, s2) + 1024) <= smem_cap) stages = s2;
-    }
-    if (stages > a.nkb) stages = a.nkb < 2 ? 2 : a.nkb;
-    ESR_REQUIRE(tc_smem_bytes(a.npad, stages) <= smem_cap, "conv_tc: npad=%d needs %zu B of shared memory, the device allows %zu",
-                a.npad, tc_smem_bytes(a.npad, stages), smem_cap);
-    a.stages = stages;
+    const uint32_t a_box = tc_a_box_bytes(TW, TH, d.ntaps);
+    ESR_REQUIRE(tc_rings(a.npad, a_box, d.ntaps == 9 ? 3 : 1, smem_cap, &a.a_stages, &a.b_stages),
+                "conv_tc: npad=%d needs %zu B of shared memory, the device allows %zu", a.npad, tc_smem_bytes(a.npad, a_box, 1, 2),
+                smem_cap);
     a.bias = d.bias;
     a.act = d.act; a.act_from = d.act_from; a.res_mode = d.res_mode; a.epi_mode = d.epi_mode;
     if (d.res_mode != RES_NONE) {
@@ -342,7 +392,7 @@ template <int NP>
 static int launch_np(const ConvTCArgs &a, cudaStream_t st)
 {
     static int max_set = 0;
-    const size_t smem = tc_smem_bytes(NP, a.stages);
+    const size_t smem = tc_smem_bytes(NP, tc_a_box_bytes(a.TW, a.TH, a.ntaps), a.a_stages, a.b_stages);
     if ((int)smem > max_set) {
         ESR_CUDA_CHECK(cudaFuncSetAttribute(k_conv_tc<NP>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         max_set = (int)smem;
@@ -380,7 +430,7 @@ int conv_tc_launch(const ConvTCArgs &a, cudaStream_t st)
     return ESR_EINVAL;
 }
 
-struct GruChainPlan { ConvTCArgs *args = nullptr; unsigned int *ctr = nullptr; int nphase = 0, stages = 2; unsigned grid = 0; size_t smem = 0; };
+struct GruChainPlan { ConvTCArgs *args = nullptr; unsigned int *ctr = nullptr; int nphase = 0, na = 2, nb = 2; unsigned grid = 0; size_t smem = 0; };
 
 int gru_chain_prepare(const std::vector<ConvTCArgs> &zr, const std::vector<ConvTCArgs> &go, void **plan_out)
 {
@@ -394,11 +444,13 @@ int gru_chain_prepare(const std::vector<ConvTCArgs> &zr, const std::vector<ConvT
         ph.push_back(zr[g]); ph.push_back(go[g]);
     }
     p->nphase = (int)ph.size();
+    // both phases share one layout: A boxes of the (common) tile shape, B slots of the wider (128) phase
     const size_t cap = (size_t)dev_info().max_smem_optin;
-    int stages = 6;
-    while (stages > 2 && tc_smem_bytes(128, stages) > cap) --stages;
-    p->stages = stages;
-    p->smem = tc_smem_bytes(128, stages);
+    const uint32_t a_box = tc_a_box_bytes(zr[0].TW, zr[0].TH, zr[0].ntaps);
+    if (!tc_rings(128, a_box, zr[0].ntaps == 9 ? 3 : 1, cap, &p->na, &p->nb)) {
+        delete p; set_error("gru_chain: the rings do not fit in shared memory"); return ESR_EINVAL;
+    }
+    p->smem = tc_smem_bytes(128, a_box, p->na, p->nb);
     cudaError_t e = cudaFuncSetAttribute(k_gru_chain, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)p->smem);
     int per_sm = 0;
     if (e == cudaSuccess) e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_gru_chain, TC_THREADS, p->smem);
@@ -427,7 +479,7 @@ int gru_chain_launch(void *plan, cudaStream_t st)
     at[0].id = cudaLaunchAttributeCooperative;
     at[0].val.cooperative = 1;
     cfg.attrs = at; cfg.numAttrs = 1;
-    ESR_CUDA_CHECK(cudaLaunchKernelEx(&cfg, k_gru_chain, (const ConvTCArgs *)p->args, p->nphase, p->stages, p->ctr));
+    ESR_CUDA_CHECK(cudaLaunchKernelEx(&cfg, k_gru_chain, (const ConvTCArgs *)p->args, p->nphase, p->na, p->nb, p->ctr));
     esr::count_launch();
     return ESR_OK;
 }

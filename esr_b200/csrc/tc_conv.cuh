@@ -22,13 +22,13 @@ constexpr int TC_MAX_SRC = 3;
 
 // Everything one launch needs.  Passed to the kernel by value (__grid_constant__).
 struct ConvTCArgs {
-    CUtensorMap amap[TC_MAX_SRC];   // 5-D maps over the source split tensors (C, W, H, img, plane), box (64, TW, TH, 1, 1)
+    CUtensorMap amap[TC_MAX_SRC];   // 5-D maps over the source split tensors (C, W, H, img, plane), box (64, TW, tc_box_h, 1, 1)
     CUtensorMap bmap;               // 3-D map over packed weights (64, npad, 2*nkb), box (64, npad, 1)
     const int *src_img[TC_MAX_SRC]; // output image -> source image (nullptr = identity)
     int chunk_end[TC_MAX_SRC];      // cumulative number of 64-channel chunks after source s
     int n_src, ntaps, nkb, npad, cout;
     int H, W, TW, TH, tiles_x, tiles_y, n_img;
-    int stages;
+    int a_stages, b_stages;         // ring depths: A boxes (one per chunk and dx), B slots (one per tap)
     // epilogue
     const float *bias;              // [npad]
     int act, act_from, res_mode, epi_mode;
@@ -69,6 +69,11 @@ struct ConvTCDesc {
 };
 
 static inline int tc_npad(int cout) { return (cout + 15) / 16 * 16; }
+// Rows of one A box: a 3x3 layer's box has the tile's TH rows plus a halo row above and below, so that its three dy taps
+// read it at row offsets 0, TW and 2 TW; a 1x1 layer's box is the tile.
+__host__ __device__ inline int tc_box_h(int TH, int ntaps) { return ntaps == 9 ? TH + 2 : TH; }
+// bytes of one A box, both planes (64 channels = 128 bytes per pixel and plane)
+__host__ __device__ inline uint32_t tc_a_box_bytes(int TW, int TH, int ntaps) { return 2u * 128u * (uint32_t)(TW * tc_box_h(TH, ntaps)); }
 static inline int tc_nkb(int cin_total, int ntaps) { return cin_total / 64 * ntaps; }
 static inline size_t tc_packed_weight_bytes(int cout, int cin_total, int ntaps)
 {
