@@ -69,6 +69,7 @@ SIGNATURES.update({
     "esr_net_create": (c_int, [ctypes.POINTER(c_void_p), c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_size_t, c_void_p]),
     "esr_net_destroy": (c_int, [c_void_p]),
     "esr_net_reset_states": (c_int, [c_void_p, c_void_p]),
+    "esr_net_reset_sample_states": (c_int, [c_void_p, c_int, c_void_p]),
     "esr_net_forward": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
     "esr_net_forward_profiled": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p,
                                          c_void_p, c_void_p, c_void_p, c_void_p]),
@@ -84,6 +85,8 @@ SIGNATURES.update({
     "esr_gather_events_aug": (c_int, [c_void_p] * 7 + [c_int, c_int, c_int, c_i64] + [c_void_p] * 5),
     "esr_metrics_workspace_bytes": (c_size_t, [c_int, c_int, c_int, c_int]),
     "esr_metrics_planes": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, ctypes.c_double, c_void_p, c_void_p, c_size_t, c_void_p]),
+    "esr_render_workspace_bytes": (c_size_t, [c_int, c_int, c_int]),
+    "esr_render_event_cnt": (c_int, [c_void_p] + [c_int] * 7 + [c_void_p, c_void_p, c_void_p, c_size_t, c_void_p]),
 })
 
 SIGNATURES.update({

@@ -648,6 +648,22 @@ extern "C" int esr_net_reset_states(esr_net_t net, esr_stream_t stream)
     return ESR_OK;
 }
 
+extern "C" int esr_net_reset_sample_states(esr_net_t net, int b, esr_stream_t stream)
+{
+    ESR_REQUIRE(net, "esr_net_reset_sample_states: null net");
+    Net &n = *(Net *)net;
+    ESR_REQUIRE(b >= 0 && b < n.B, "esr_net_reset_sample_states: sample %d out of [0, %d)", b, n.B);
+    // slot 0 holds the forward-direction state of sample b in image b and the reverse-direction one in image B + b
+    const size_t img = (size_t)n.h * n.w * 64;
+    const size_t cnt = img * sizeof(__nv_bfloat16);
+    __nv_bfloat16 *s0 = view_imgs(n.hs, 0).base;
+    for (int i : {b, n.B + b}) {
+        ESR_CUDA_CHECK(cudaMemsetAsync(s0 + (size_t)i * img, 0, cnt, (cudaStream_t)stream));
+        ESR_CUDA_CHECK(cudaMemsetAsync(s0 + n.hs.plane() + (size_t)i * img, 0, cnt, (cudaStream_t)stream));
+    }
+    return ESR_OK;
+}
+
 extern "C" int esr_net_forward(esr_net_t net, const float *input, const int32_t *in_img, float *output, esr_stream_t stream)
 {
     ESR_REQUIRE(net && input && output, "esr_net_forward: null pointer");

@@ -29,6 +29,11 @@ FLOAT_DATA_RANGE = 2.0
 def plane_stats(pred, tgt, win=WIN, data_range=FLOAT_DATA_RANGE):
     """pred, tgt: CUDA fp32 [..., H, W] of equal shape -> CPU float64 [n_planes, 6]:
     {sum |d|, sum d^2, max tgt, min tgt, SSIM-map sum over the valid region, valid pixel count} per plane."""
+    return plane_stats_device(pred, tgt, win, data_range).cpu()
+
+
+def plane_stats_device(pred, tgt, win=WIN, data_range=FLOAT_DATA_RANGE):
+    """plane_stats left on the device (no synchronisation): CUDA float64 [n_planes, 6]."""
     if not (pred.is_cuda and tgt.is_cuda):
         raise _lib.ESRError("esr_b200.metrics needs CUDA tensors (no CPU fallback)")
     assert pred.shape == tgt.shape and pred.dim() >= 2
@@ -43,7 +48,7 @@ def plane_stats(pred, tgt, win=WIN, data_range=FLOAT_DATA_RANGE):
         stats = torch.zeros((n, 6), dtype=torch.float64, device=p.device)
         _lib.check(L.esr_metrics_planes(_lib.ptr(p), _lib.ptr(t), n, H, W, int(win), float(data_range), _lib.ptr(stats),
                                         _lib.ptr(ws), nbytes, _lib.stream_ptr()), "esr_metrics_planes")
-    return stats.cpu()
+    return stats
 
 
 def l1(pred, tgt):
@@ -119,3 +124,12 @@ def evaluate(pred, tgt):
     out["ssim"] = sum(ss) / B
     out["psnr"] = sum(ps) / B
     return out
+
+
+def evaluate_from_stats(s, shape):
+    """evaluate() of ONE sample from its per-plane statistics s [C, 6] (CPU float64) and its shape (C, H, W), C > 1:
+    the same arithmetic, so a batch's statistics computed once give every sample's values bit for bit."""
+    C, H, W = shape
+    assert C > 1 and s.shape[0] == C
+    a, p = _reference_reduce(s, (C, H, W))
+    return {"l1": float(s[:, 0].sum()) / (C * H * W), "mse": float(s[:, 1].sum()) / (C * H * W), "ssim": a, "psnr": p}

@@ -194,6 +194,18 @@ class DeepRecurrNet(nn.Module):
             with torch.cuda.device(p.ws.device):
                 _lib.check(_lib.lib().esr_net_reset_states(p.handle, _lib.stream_ptr()), "esr_net_reset_states")
 
+    def reset_sample_states(self, indices):
+        """Forget the carried ConvGRU states of the batch samples `indices` only (of every cached inference plan whose batch
+        holds them); the other samples keep theirs.  Lets a batch of independent recordings start a new one in one slot."""
+        idx = [int(i) for i in indices]
+        for p in self._plans.values():
+            B = p.key[0]
+            with torch.cuda.device(p.ws.device):
+                for b in idx:
+                    if not 0 <= b < B:
+                        continue
+                    _lib.check(_lib.lib().esr_net_reset_sample_states(p.handle, b, _lib.stream_ptr()), "esr_net_reset_sample_states")
+
     def states(self, B, L, H, W):
         """The carried states [h_fwd, h_rev] (each Bx64xhxw) of the plan for this shape -- the reference's
         `time_propagate.states`."""

@@ -202,6 +202,10 @@ int esr_net_create(esr_net_t *net, int B, int N, int L, int H, int W, void *blob
                    esr_stream_t stream);
 int esr_net_destroy(esr_net_t net);
 int esr_net_reset_states(esr_net_t net, esr_stream_t stream);
+/* Zero the carried states of sample b alone (both directions: images b and B + b of the state slot, both split planes) with
+ * memsets on `stream`; graph-capturable.  The other samples' states are untouched, so a batch can start a new recording
+ * in one slot while the others continue theirs. */
+int esr_net_reset_sample_states(esr_net_t net, int b, esr_stream_t stream);
 int esr_net_forward(esr_net_t net, const float *input, const int32_t *in_img, float *output, esr_stream_t stream);
 /* Same as esr_net_forward, but brackets every kernel launch with CUDA events on `stream`, synchronises, and reports
  * per-launch {class (0 tensor-core conv, 1 CUDA-core conv, 2 element-wise/sampling, 3 cooperative ConvGRU chain),
@@ -307,6 +311,17 @@ int esr_adam_step_dev(float *param, const float *grad, float *exp_avg, float *ex
 size_t esr_metrics_workspace_bytes(int n_planes, int H, int W, int win);
 int esr_metrics_planes(const float *pred, const float *tgt, int n_planes, int H, int W, int win, double data_range, double *stats,
                        void *workspace, size_t workspace_bytes, esr_stream_t stream);
+
+/* ---------------------------------------------------------------------------------------------
+ * Event-count images of the evaluation script (myutils/vis_events/matplotlib_plot_events.py:125-248, plot_event_cnt with
+ * is_save=False) for B images at once.  cnt: fp32 [B, 2, H, W] (0 positive, 1 negative), H * W < 2^24.
+ * color_scheme: 0 gray, 1 green_red, 2 blue_red.  out: uint8 [B, H, W, 3] (gray: [B, H, W]); channels in BGR order when
+ * bgr != 0 (use_opencv=True), else RGB (the script's cv2.cvtColor(BGR2RGB)).  The 1st / 99th percentiles of every plane
+ * are numpy 2.x np.percentile's float32 values, from a radix select; percentiles (optional, device) receives them as
+ * fp32 [B, 2 planes, 2] = {p1, p99}.  workspace: esr_render_workspace_bytes(B, H, W) bytes of device memory. */
+size_t esr_render_workspace_bytes(int B, int H, int W);
+int esr_render_event_cnt(const float *cnt, int B, int H, int W, int color_scheme, int black_background, int is_norm, int bgr,
+                         unsigned char *out, float *percentiles, void *workspace, size_t workspace_bytes, esr_stream_t stream);
 
 /* ---------------------------------------------------------------------------------------------
  * Columnar event reader, device side (SURVEY 8f rank 2).  Replaces, for whole batches of frames:
