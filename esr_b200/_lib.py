@@ -83,6 +83,7 @@ SIGNATURES.update({
     "esr_gather_events": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_i64, c_void_p, c_void_p,
                                   c_void_p, c_void_p, c_void_p]),
     "esr_gather_events_aug": (c_int, [c_void_p] * 7 + [c_int, c_int, c_int, c_i64] + [c_void_p] * 5),
+    "esr_encode_frames_multi": (c_int, [c_void_p, c_void_p, c_int, c_i64] + [c_int] * 4 + [c_void_p] * 3),
     "esr_metrics_workspace_bytes": (c_size_t, [c_int, c_int, c_int, c_int]),
     "esr_metrics_planes": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, ctypes.c_double, c_void_p, c_void_p, c_size_t, c_void_p]),
     "esr_render_workspace_bytes": (c_size_t, [c_int, c_int, c_int]),

@@ -71,9 +71,92 @@ k_gather_events(const short *__restrict__ xs, const short *__restrict__ ys, cons
     }
 }
 
+// ---------------------------------------------------------------------------------------------------------------------
+// Columns of many recordings -> count banks in one pass (the batch of HDF5DataLoaderSequence, dataloader/h5dataloader.py:
+// 180-233, whose samples come from different SequenceDatasets of one ConcatDataset).  The same arithmetic as
+// k_gather_events followed by k_scatter_cnt with writeback == 2 (events.cu), without the fp32 SoA in between:
+//   x, y (int16) and p (float64) are read once per event (12 B; ts is not read), cast to fp32 and flipped in registers;
+//   LR bank: the event as it is; lifted bank: x / W * kW, y / H * kH with two fp32 roundings (h5dataset.py:515, 526);
+//   out of range: positive weight dropped; the negative weight lands on neg[0, 0] unless the frame holds more than 3 events
+//   (create_stack_encoding zeroed x, y and p first, h5dataset.py:337-354, encodings.py:219-220, 251-256);
+//   a paused frame is the reference's one zero event (p = 0): it adds nothing, so its block returns at once.
+// Counts are fp32 sums of p * p, exact and order-independent for p = +-1, so the banks equal the two-step path bit for bit.
+struct FrameDesc {
+    long long start, len;     // rows [start, start + len) of recording rec's columns
+    int rec, xform;           // xform: the transform word of k_gather_events (bit 3 = paused)
+};
+
+__device__ __forceinline__ void scatter_pn(float *__restrict__ img, int H, int W, float x, float y, float vpos, float vneg, bool many)
+{
+    if ((x >= (float)W) | (x < 0.0f) | (y >= (float)H) | (y < 0.0f)) {
+        x = 0.0f; y = 0.0f; vpos = 0.0f;
+        if (many) vneg = 0.0f;
+    }
+    const size_t pix = (size_t)(long long)y * W + (size_t)(long long)x;     // .long(): truncation toward zero
+    if (vpos != 0.0f) atomicAdd(img + pix, vpos);
+    if (vneg != 0.0f) atomicAdd(img + (size_t)H * W + pix, vneg);
+}
+
+// grid (frames, blocks per frame); cols = [R][3] addresses of the xs, ys, ps columns of recording r (pinned host or HBM)
+template <bool LIFT>
+__global__ void __launch_bounds__(256)
+k_encode_frames_multi(const unsigned long long *__restrict__ cols, const FrameDesc *__restrict__ desc, int H, int W, int kH, int kW,
+                      float *__restrict__ out, float *__restrict__ out_hr)
+{
+    const unsigned f = blockIdx.x;
+    const FrameDesc d = desc[f];
+    if (d.xform & 8) return;
+    const short *__restrict__ xs = reinterpret_cast<const short *>(cols[3 * d.rec]) + d.start;
+    const short *__restrict__ ys = reinterpret_cast<const short *>(cols[3 * d.rec + 1]) + d.start;
+    const double *__restrict__ ps = reinterpret_cast<const double *>(cols[3 * d.rec + 2]) + d.start;
+    const bool many = d.len > 3;
+    const float wm1 = (float)(W - 1), hm1 = (float)(H - 1);
+    float *img = out + (size_t)f * 2 * H * W;
+    float *img_hr = LIFT ? out_hr + (size_t)f * 2 * kH * kW : nullptr;
+    for (long long i = (long long)blockIdx.y * blockDim.x + threadIdx.x; i < d.len; i += (long long)gridDim.y * blockDim.x) {
+        float x = (float)xs[i], y = (float)ys[i], p = (float)ps[i];
+        if (d.xform & 1) x = __fsub_rn(wm1, x);
+        if (d.xform & 2) y = __fsub_rn(hm1, y);
+        if (d.xform & 4) p = -p;
+        const float vpos = __fmul_rn(p, p < 0.0f ? 0.0f : p);
+        const float vneg = __fmul_rn(p, p > 0.0f ? 0.0f : p);
+        scatter_pn(img, H, W, x, y, vpos, vneg, many);
+        if (LIFT)
+            scatter_pn(img_hr, kH, kW, __fmul_rn(__fdiv_rn(x, (float)W), (float)kW), __fmul_rn(__fdiv_rn(y, (float)H), (float)kH),
+                       vpos, vneg, many);
+    }
+}
+
 } // namespace esr
 
 using namespace esr;
+
+static_assert(sizeof(FrameDesc) == sizeof(esr_frame_desc), "esr_frame_desc layout");
+
+extern "C" int esr_encode_frames_multi(const uint64_t *cols, const esr_frame_desc *desc, int n_frames, int64_t max_len, int H, int W,
+                                       int kH, int kW, float *out_cnt, float *out_scaled_cnt, esr_stream_t stream)
+{
+    ESR_REQUIRE(n_frames >= 0 && H > 0 && W > 0 && H < (1 << 23) && W < (1 << 23) && out_cnt && max_len >= 0,
+                "esr_encode_frames_multi: bad arguments");
+    ESR_REQUIRE(!out_scaled_cnt || (kH > 0 && kW > 0), "esr_encode_frames_multi: bad lifted resolution");
+    cudaStream_t st = (cudaStream_t)stream;
+    if (n_frames == 0) return ESR_OK;
+    ESR_CUDA_CHECK(cudaMemsetAsync(out_cnt, 0, sizeof(float) * (size_t)n_frames * 2 * H * W, st));
+    if (out_scaled_cnt) ESR_CUDA_CHECK(cudaMemsetAsync(out_scaled_cnt, 0, sizeof(float) * (size_t)n_frames * 2 * kH * kW, st));
+    if (max_len == 0) return ESR_OK;
+    ESR_REQUIRE(cols && desc, "esr_encode_frames_multi: null tables");
+    // as esr_scatter_cnt: ~8 events per thread for the longest frame, capped for huge frames; frames on grid x (up to 2^31 - 1)
+    const int64_t by = max((int64_t)1, min(ceil_div64(max_len, 256 * 8), min((int64_t)dev_info().sm_count * 16, (int64_t)65535)));
+    const dim3 grid((unsigned)n_frames, (unsigned)by);
+    const FrameDesc *dd = reinterpret_cast<const FrameDesc *>(desc);
+    const unsigned long long *cc = reinterpret_cast<const unsigned long long *>(cols);
+    if (out_scaled_cnt)
+        k_encode_frames_multi<true><<<grid, 256, 0, st>>>(cc, dd, H, W, kH, kW, out_cnt, out_scaled_cnt);
+    else
+        k_encode_frames_multi<false><<<grid, 256, 0, st>>>(cc, dd, H, W, 0, 0, out_cnt, nullptr);
+    ESR_LAUNCH_CHECK();
+    return ESR_OK;
+}
 
 extern "C" int esr_ts_search(const double *ts, int64_t n, const double *queries, int64_t nq, int64_t *out, esr_stream_t stream)
 {

@@ -7,7 +7,10 @@ install() registers, under the module names the reference imports (SURVEY.md 8b)
   `dataloader.cython_cnt2event.cnt2event`          -> esr_b200.cnt2event       (cnt2event_api.py:1)
   `dataloader.cython_event_redistribute.event_redistribute` -> esr_b200.event_redistribute (encodings.py:5)
   `models.model` : a module exposing DeepRecurrNet  -> esr_b200.model          (train_ours_cnt_seq.py:20, infer_ours_cnt.py:14)
-and, optionally (patch_encodings=True), replaces the hot functions of an already imported `dataloader.encodings`.
+and, optionally (patch_encodings=True), replaces the hot functions of an already imported `dataloader.encodings`, and
+(patch_loader=True) registers `dataloader.h5dataloader` exposing esr_b200.loader.HDF5DataLoaderSequence and an
+HDF5DataLoader that raises ESRError when constructed (train_ours_cnt_seq.py:18 imports both names; the per-frame
+H5Dataset loader is not served).
 """
 import importlib.util
 import sys
@@ -33,7 +36,7 @@ def _package(name):
     return m
 
 
-def install(patch_models=True, patch_encodings=False):
+def install(patch_models=True, patch_encodings=False, patch_loader=False):
     from . import cnt2event, dcn_v2_ext, event_redistribute, model
     sys.modules["_ext"] = dcn_v2_ext
     _package("dataloader.cython_cnt2event").cnt2event = cnt2event
@@ -54,3 +57,19 @@ def install(patch_models=True, patch_encodings=False):
         ref = sys.modules["dataloader.encodings"]
         for name in ("events_to_image", "events_to_channels", "cython_event_redistribute", "multiprocess_cython", "stack2cnt"):
             setattr(ref, name, getattr(encodings, name))
+    if patch_loader:
+        from . import loader
+        m = types.ModuleType("dataloader.h5dataloader")
+        m.HDF5DataLoaderSequence = loader.HDF5DataLoaderSequence
+        m.HDF5DataLoader = _HDF5DataLoader
+        sys.modules["dataloader.h5dataloader"] = m
+        _package("dataloader").h5dataloader = m
+
+
+class _HDF5DataLoader:
+    """dataloader/h5dataloader.py:HDF5DataLoader (one H5Dataset item per batch entry) is not served: constructing it raises."""
+
+    def __init__(self, *args, **kwargs):
+        from ._lib import ESRError
+        raise ESRError("HDF5DataLoader (per-frame H5Dataset batches) is not implemented; train from "
+                       "HDF5DataLoaderSequence (esr_b200.loader)")

@@ -217,7 +217,7 @@ def augmentation_enabled(config):
                 config.get("sequence", {}).get("pause", {}).get("enabled", False))
 
 
-def draw_decisions(config, n, L):
+def draw_decisions(config, n, L, rng=None):
     """The random decisions of n consecutive SequenceDataset.__getitem__ calls of L frames each, drawn from the module-level
     `random` generator as the reference draws them, leaving the generator where the reference leaves it (the next
     sequence's seed depends on that).  The reference's calls:
@@ -238,8 +238,12 @@ def draw_decisions(config, n, L):
     milliseconds per batch.  Items that never reseed (augmentation off) leave the pause draws successive values of the
     global stream, drawn here from it directly.
 
+    rng: a random.Random to draw from instead of the module-level generator (a DataLoader worker's own `random`, reseeded
+    base_seed + worker id by torch/utils/data/_utils/worker.py); None draws from and advances the module-level one.
+
     -> {"seed": int64 [n], "flips": int32 [n] (FLIP_X | FLIP_Y | NEGATE_P bits; the same for every frame and for input and
     ground truth), "paused": bool [n, L]}."""
+    gen = random if rng is None else rng
     aug = config.get("data_augment", {})
     mechs = list(aug.get("augment", [])) if aug.get("enabled", False) else []
     probs = aug.get("augment_prob", [])
@@ -258,7 +262,7 @@ def draw_decisions(config, n, L):
 
     seeds, flips, paused = np.zeros(n, np.int64), np.zeros(n, np.int32), np.zeros((n, L), bool)
     for s in range(n):
-        seed = random.randint(0, 2**32)
+        seed = gen.randint(0, 2**32)
         seeds[s] = seed
         bits = 0
         for i, m in enumerate(mechs):                    # augment_event; input and ground truth flip alike
@@ -275,12 +279,12 @@ def draw_decisions(config, n, L):
         for f in range(1, L):
             if pause_on:
                 if last is None:
-                    u = random.random()
+                    u = gen.random()
                 p = u < (p_paused if p else p_run)
             paused[s, f] = p
         if last is not None:                             # the state the sequence's last item leaves behind
-            random.seed(seed + last)
-            random.random()
+            gen.seed(seed + last)
+            gen.random()
     return {"seed": seeds, "flips": flips, "paused": paused}
 
 

@@ -344,6 +344,23 @@ int esr_gather_events_aug(const int16_t *xs, const int16_t *ys, const double *ts
                           const int64_t *off, const int32_t *xform, int W, int H, int n_frames, int64_t max_len,
                           float *out_xs, float *out_ys, float *out_ts, float *out_ps, esr_stream_t stream);
 
+/* Columns of many recordings -> count banks, one launch per event stream: the batch of HDF5DataLoaderSequence
+ * (dataloader/h5dataloader.py:180-233: SequenceDatasets joined by ConcatDataset, stacked by custom_collate), each sample
+ * encoded as H5Dataset.__getitem__ does (h5dataset.py:337-354, 508-528) with SequenceDataset's flips and pauses (:652-670,
+ * 769-789).  Equal, bit for bit, to esr_gather_events_aug followed by esr_scatter_cnt(writeback = 2) per frame: without and
+ * (out_scaled_cnt) with the x / W * kW, y / H * kH lift.
+ *   cols: device table [R][3] of the addresses of recording r's int16 xs, int16 ys and float64 ps columns (pinned host
+ *         memory or HBM); desc: device table [n_frames]; frame f = rows [start, start + len) of recording rec, transformed
+ *         by xform (the word of esr_gather_events_aug; bit 3 paused: the frame adds nothing, len should be 1);
+ *   H, W: the stream's resolution (flips and out_cnt [n_frames, 2, H, W]); kH, kW: out_scaled_cnt [n_frames, 2, kH, kW];
+ *   max_len: the longest len (grid sizing).  Both banks are zeroed by the call.  Up to 2^31 - 1 frames. */
+typedef struct {
+    int64_t start, len;
+    int32_t rec, xform;
+} esr_frame_desc;
+int esr_encode_frames_multi(const uint64_t *cols, const esr_frame_desc *desc, int n_frames, int64_t max_len, int H, int W, int kH,
+                            int kW, float *out_cnt, float *out_scaled_cnt, esr_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif
