@@ -86,6 +86,12 @@ SIGNATURES.update({
     "esr_encode_frames_multi": (c_int, [c_void_p, c_void_p, c_int, c_i64] + [c_int] * 4 + [c_void_p] * 3),
     "esr_metrics_workspace_bytes": (c_size_t, [c_int, c_int, c_int, c_int]),
     "esr_metrics_planes": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, ctypes.c_double, c_void_p, c_void_p, c_size_t, c_void_p]),
+    "esr_lpips_param_bytes": (c_size_t, []),
+    "esr_lpips_pack_params": (c_int, [c_void_p, c_void_p, c_void_p]),
+    "esr_lpips_workspace_bytes": (c_size_t, [c_int, c_int, c_int]),
+    "esr_lpips_create": (c_int, [ctypes.POINTER(c_void_p), c_int, c_int, c_int, c_void_p, c_void_p, c_size_t]),
+    "esr_lpips_destroy": (c_int, [c_void_p]),
+    "esr_lpips_forward": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p]),
     "esr_render_workspace_bytes": (c_size_t, [c_int, c_int, c_int]),
     "esr_render_event_cnt": (c_int, [c_void_p] + [c_int] * 7 + [c_void_p, c_void_p, c_void_p, c_size_t, c_void_p]),
 })

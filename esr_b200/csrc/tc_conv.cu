@@ -1,4 +1,4 @@
-// tc_conv.cu -- 3x3 / 1x1 convolution as an implicit GEMM on the Hopper tensor cores (sm_90a, wgmma).
+// tc_conv.cu -- 3x3 / 1x1 (and LPIPS's 5x5) convolution as an implicit GEMM on the Hopper tensor cores (sm_90a, wgmma).
 //
 //   D[128 pixels, Cout] += A[128 pixels, 64 ch of one tap] * B[Cout, 64]^T      per K-block (tap x 64-channel chunk)
 //
@@ -102,14 +102,18 @@ __device__ __forceinline__ void tc_init_barriers(const TcSmem &m)
     __syncthreads();
 }
 
-template <int NP>
+// KS = 0: 3x3 or 1x1 (a.ntaps 9 or 1); KS = 5: 5x5, pad 2 (a.ntaps 25) -- one box of TW x (TH + 4) pixels per (chunk, dx),
+// read by the five dy taps, and the packing's order chunk * 25 + 5 (dy + 2) + dx + 2.
+template <int NP, int KS = 0>
 __device__ __forceinline__ void conv_tiles(const ConvTCArgs &a, int tile0, int step, const TcSmem &m, TcRing &ring)
 {
+    static_assert(KS == 0 || KS == 5, "conv_tiles: KS is 0 (3x3 / 1x1) or 5");
+    constexpr bool k5 = KS == 5;
     constexpr uint32_t b_bytes = (uint32_t)NP * 128u;                  // one plane of one tap's weights
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int tiles_per_img = a.tiles_x * a.tiles_y, n_tiles = a.n_img * tiles_per_img;
     const bool k3 = a.ntaps == 9;
-    const int taps = k3 ? 3 : 1, nbox = a.nkb / taps;                  // dy taps per A box, A boxes per tile
+    const int taps = k5 ? 5 : k3 ? 3 : 1, nbox = a.nkb / taps;         // dy taps per A box, A boxes per tile
     const uint32_t a_plane = m.a_box / 2;
 
     if (warp == 8) {
@@ -121,7 +125,8 @@ __device__ __forceinline__ void conv_tiles(const ConvTCArgs &a, int tile0, int s
                 const int y0 = (trem / a.tiles_x) * a.TH, x0 = (trem % a.tiles_x) * a.TW;
                 int src = 0, chunk_base = 0;
                 for (int bx = 0; bx < nbox; ++bx) {
-                    const int gchunk = k3 ? bx / 3 : bx, dx = k3 ? bx - 3 * gchunk - 1 : 0;
+                    const int gchunk = k5 ? bx / 5 : k3 ? bx / 3 : bx, dx = k5 ? bx - 5 * gchunk - 2 : k3 ? bx - 3 * gchunk - 1 : 0;
+                    const int ytop = y0 - (k5 ? 2 : k3 ? 1 : 0);
                     while (gchunk >= a.chunk_end[src]) { chunk_base = a.chunk_end[src]; ++src; }
                     const int cc = gchunk - chunk_base, istep = a.chunk_img_step[src];
                     const int simg = (a.src_img[src] ? a.src_img[src][img] : img) + cc * istep;
@@ -130,11 +135,12 @@ __device__ __forceinline__ void conv_tiles(const ConvTCArgs &a, int tile0, int s
                     mbar_wait(m.a_empty(sa), ring_phase(ca, m.na) ^ 1u);
                     mbar_expect_tx(m.a_full(sa), m.a_box);
                     const uint32_t as = m.a_ring + sa * m.a_box;
-                    tma_load_5d(&a.amap[src], m.a_full(sa), as, c0, x0 + dx, y0 - (k3 ? 1 : 0), simg, 0);
-                    tma_load_5d(&a.amap[src], m.a_full(sa), as + a_plane, c0, x0 + dx, y0 - (k3 ? 1 : 0), simg, 1);
+                    tma_load_5d(&a.amap[src], m.a_full(sa), as, c0, x0 + dx, ytop, simg, 0);
+                    tma_load_5d(&a.amap[src], m.a_full(sa), as + a_plane, c0, x0 + dx, ytop, simg, 1);
                     ca = ring_next(ca, m.na);
                     for (int t = 0; t < taps; ++t) {
-                        const int kb = k3 ? gchunk * 9 + 3 * t + dx + 1 : gchunk;   // the packing's order: chunk * 9 + 3 (dy + 1) + dx + 1
+                        // the packing's order: chunk * 9 + 3 (dy + 1) + dx + 1 (5x5: chunk * 25 + 5 (dy + 2) + dx + 2)
+                        const int kb = k5 ? gchunk * 25 + 5 * t + dx + 2 : k3 ? gchunk * 9 + 3 * t + dx + 1 : gchunk;
                         const uint32_t sb = ring_slot(cb, m.nb);
                         mbar_wait(m.b_empty(sb), ring_phase(cb, m.nb) ^ 1u);
                         mbar_expect_tx(m.b_full(sb), 2u * b_bytes);
@@ -222,15 +228,16 @@ __device__ __forceinline__ void conv_tiles(const ConvTCArgs &a, int tile0, int s
 }
 
 // one layer: grid = min(tiles, resident CTAs); CTA b takes tiles b, b + gridDim.x, ...
-template <int NP>
+template <int NP, int KS = 0>
 __global__ void __launch_bounds__(TC_THREADS, 1) k_conv_tc(const __grid_constant__ ConvTCArgs a)
 {
     PDL_LAUNCH_DEPENDENTS();
-    const TcSmem m = tc_smem_layout(NP, tc_a_box_bytes(a.TW, a.TH, a.ntaps), a.a_stages, a.b_stages);
+    const uint32_t a_box = KS == 5 ? tc_a_box_bytes5(a.TW, a.TH) : tc_a_box_bytes(a.TW, a.TH, a.ntaps);
+    const TcSmem m = tc_smem_layout(NP, a_box, a.a_stages, a.b_stages);
     tc_init_barriers(m);
     PDL_WAIT();                      // everything above is CTA-local set-up; global memory only from here on
     TcRing ring;
-    conv_tiles<NP>(a, blockIdx.x, gridDim.x, m, ring);
+    conv_tiles<NP, KS>(a, blockIdx.x, gridDim.x, m, ring);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -327,7 +334,7 @@ int conv_tc_prepare(const ConvTCDesc &d, ConvTCArgs *args)
     ConvTCArgs &a = *args;
     memset(&a, 0, sizeof(a));
     ESR_REQUIRE(d.n_src >= 1 && d.n_src <= TC_MAX_SRC, "conv_tc: n_src=%d", d.n_src);
-    ESR_REQUIRE(d.ntaps == 9 || d.ntaps == 1, "conv_tc: ntaps=%d", d.ntaps);
+    ESR_REQUIRE(d.ntaps == 9 || d.ntaps == 1 || d.ntaps == 25, "conv_tc: ntaps=%d", d.ntaps);
     const int H = d.src[0].H, W = d.src[0].W;
     int chunks = 0;
     // tile shape: 128 pixels, 16 x 8 (8 x 16 on images narrower than 12, so that at most half a tile is wasted).  A 3x3 box of
@@ -348,7 +355,7 @@ int conv_tc_prepare(const ConvTCDesc &d, ConvTCArgs *args)
         a.chunk_end[s] = chunks;
         a.chunk_img_step[s] = d.chunk_img_step[s];
         a.src_img[s] = d.src_img[s];
-        int rc = make_amap(t, TW, tc_box_h(TH, d.ntaps), &a.amap[s]);
+        int rc = make_amap(t, TW, tc_conv_box_h(TH, d.ntaps), &a.amap[s]);
         if (rc) return rc;
     }
     for (int s = d.n_src; s < TC_MAX_SRC; ++s) a.chunk_end[s] = 1 << 30;
@@ -361,8 +368,8 @@ int conv_tc_prepare(const ConvTCDesc &d, ConvTCArgs *args)
     a.tiles_x = (W + TW - 1) / TW; a.tiles_y = (H + TH - 1) / TH; a.n_img = d.n_img;
     // Ring depths: as many slots as fit beside one CTA per SM (two 40 KB A boxes already rule out a second CTA).
     const size_t smem_cap = (size_t)dev_info().max_smem_optin;
-    const uint32_t a_box = tc_a_box_bytes(TW, TH, d.ntaps);
-    ESR_REQUIRE(tc_rings(a.npad, a_box, d.ntaps == 9 ? 3 : 1, smem_cap, &a.a_stages, &a.b_stages),
+    const uint32_t a_box = tc_conv_a_box(TW, TH, d.ntaps);
+    ESR_REQUIRE(tc_rings(a.npad, a_box, d.ntaps == 25 ? 5 : d.ntaps == 9 ? 3 : 1, smem_cap, &a.a_stages, &a.b_stages),
                 "conv_tc: npad=%d needs %zu B of shared memory, the device allows %zu", a.npad, tc_smem_bytes(a.npad, a_box, 1, 2),
                 smem_cap);
     a.bias = d.bias;
@@ -388,26 +395,31 @@ int conv_tc_prepare(const ConvTCDesc &d, ConvTCArgs *args)
 }
 
 // one instantiation per padded width (multiples of 16 up to 256): the accumulator is a register array of npad / 2 floats
-template <int NP>
+template <int NP, int KS = 0>
 static int launch_np(const ConvTCArgs &a, cudaStream_t st)
 {
     static int max_set = 0;
-    const size_t smem = tc_smem_bytes(NP, tc_a_box_bytes(a.TW, a.TH, a.ntaps), a.a_stages, a.b_stages);
+    const size_t smem = tc_smem_bytes(NP, tc_conv_a_box(a.TW, a.TH, a.ntaps), a.a_stages, a.b_stages);
     if ((int)smem > max_set) {
-        ESR_CUDA_CHECK(cudaFuncSetAttribute(k_conv_tc<NP>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        ESR_CUDA_CHECK(cudaFuncSetAttribute(k_conv_tc<NP, KS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         max_set = (int)smem;
     }
     int per_sm = 0;
-    ESR_CUDA_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_conv_tc<NP>, TC_THREADS, smem));
+    ESR_CUDA_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_conv_tc<NP, KS>, TC_THREADS, smem));
     const int n_tiles = a.n_img * a.tiles_x * a.tiles_y;
     const unsigned grid = (unsigned)std::max(1, std::min(n_tiles, std::max(per_sm, 1) * dev_info().sm_count));
-    ESR_CUDA_CHECK(launch_pdl(k_conv_tc<NP>, dim3(grid), dim3(TC_THREADS), smem, st, a));
+    ESR_CUDA_CHECK(launch_pdl(k_conv_tc<NP, KS>, dim3(grid), dim3(TC_THREADS), smem, st, a));
     esr::count_launch();
     return ESR_OK;
 }
 
 int conv_tc_launch(const ConvTCArgs &a, cudaStream_t st)
 {
+    if (a.ntaps == 25) {                 // 5x5: the width LPIPS's conv2 uses (AlexNet features.3, 64 -> 192)
+        if (a.npad == 192) return launch_np<192, 5>(a, st);
+        set_error("conv_tc: 5x5 taps are instantiated for npad 192 only, not %d", a.npad);
+        return ESR_EUNSUPPORTED;
+    }
     switch (a.npad) {
     case 16: return launch_np<16>(a, st);
     case 32: return launch_np<32>(a, st);
@@ -522,7 +534,7 @@ __global__ void k_pack_weight(const float *__restrict__ w0, const float *__restr
 
 int pack_conv_weight2(const float *w0, const float *w1, int cout_each, int cin, int ksz, void *dst, cudaStream_t st)
 {
-    ESR_REQUIRE(cin % 64 == 0 && (ksz == 1 || ksz == 3), "pack_conv_weight: cin=%d ksz=%d", cin, ksz);
+    ESR_REQUIRE(cin % 64 == 0 && (ksz == 1 || ksz == 3 || ksz == 5), "pack_conv_weight: cin=%d ksz=%d", cin, ksz);
     const int cout = w1 ? 2 * cout_each : cout_each;
     const int npad = tc_npad(cout), nkb = tc_nkb(cin, ksz * ksz);
     const size_t total = (size_t)nkb * npad * 64;

@@ -56,7 +56,7 @@ struct ConvTCDesc {
     int src_chunks[TC_MAX_SRC] = {0, 0, 0};
     int chunk_img_step[TC_MAX_SRC] = {0, 0, 0};
     int n_src = 1;
-    int ntaps = 9;                  // 9 (3x3, pad 1) or 1 (1x1)
+    int ntaps = 9;                  // 9 (3x3, pad 1), 1 (1x1) or 25 (5x5, pad 2; npad 192 only)
     int cout = 64;
     const void *wpacked = nullptr;  // packed by pack_conv_weight: [2][nkb][npad][64] bf16
     const float *bias = nullptr;    // [npad] fp32, zero padded
@@ -74,6 +74,11 @@ static inline int tc_npad(int cout) { return (cout + 15) / 16 * 16; }
 __host__ __device__ inline int tc_box_h(int TH, int ntaps) { return ntaps == 9 ? TH + 2 : TH; }
 // bytes of one A box, both planes (64 channels = 128 bytes per pixel and plane)
 __host__ __device__ inline uint32_t tc_a_box_bytes(int TW, int TH, int ntaps) { return 2u * 128u * (uint32_t)(TW * tc_box_h(TH, ntaps)); }
+// A 5x5 layer (ntaps 25, LPIPS's conv2) has two halo rows above and below; the kernel knows it at compile time, so the
+// 3x3 / 1x1 helpers above stay as they are and the host sizes every kind through these two.
+__host__ __device__ inline uint32_t tc_a_box_bytes5(int TW, int TH) { return 2u * 128u * (uint32_t)(TW * (TH + 4)); }
+static inline int tc_conv_box_h(int TH, int ntaps) { return ntaps == 25 ? TH + 4 : tc_box_h(TH, ntaps); }
+static inline uint32_t tc_conv_a_box(int TW, int TH, int ntaps) { return ntaps == 25 ? tc_a_box_bytes5(TW, TH) : tc_a_box_bytes(TW, TH, ntaps); }
 static inline int tc_nkb(int cin_total, int ntaps) { return cin_total / 64 * ntaps; }
 static inline size_t tc_packed_weight_bytes(int cout, int cin_total, int ntaps)
 {

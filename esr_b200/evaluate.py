@@ -23,8 +23,12 @@ images per frame.  Here:
   * `time` is device milliseconds per window from CUDA events around each model call, divided among the windows the call
     evaluated.  The reference's `time.time()` pair around an asynchronous CUDA call without a synchronise measures the
     enqueue, not the forward pass (and is in seconds).
-  * `params` is the reference's sum of parameter counts / 1e6.  The LPIPS pair (AlexNet weights are not available
-    offline) and `macs` (never updated by the reference) are left out.
+  * `params` is the reference's sum of parameter counts / 1e6.  `macs` (never updated by the reference) is left out.
+  * esr_lpips / bicubic_lpips (:85, :90) need AlexNet weights the package does not ship, so they are computed when the caller
+    passes an esr_b200.lpips.LPIPS object (lpips=...): one LPIPS pass per step over the step's esr, bicubic and gt planes
+    (gt's features computed once for both pairs), each plane repeated to three channels and the two channels' distances
+    averaged as perceptual_loss does (loss/restore.py:33-37), averaged per recording like the other keys.  Without it the
+    results hold METRIC_KEYS only.
 
 With image_dir, the five images of infer_body (:104-108) are written per evaluated frame as
 image_dir/<recording>/event_img/{lr_event_img, hr_scaled_event_img, hr_bicubic_event_img, hr_esr_event_img (of round(esr)),
@@ -43,6 +47,7 @@ from .eventstore import SequenceReader
 
 METRIC_KEYS = ("esr_l1", "esr_mse", "esr_ssim", "esr_psnr", "bicubic_l1", "bicubic_mse", "bicubic_ssim", "bicubic_psnr",
                "time", "params")
+LPIPS_KEYS = ("esr_lpips", "bicubic_lpips")
 IMAGE_KINDS = ("lr_event_img", "hr_scaled_event_img", "hr_bicubic_event_img", "hr_esr_event_img", "hr_gt_event_img")
 
 
@@ -164,11 +169,12 @@ def _steps(model, recs, B, consecutive, chunk, dev):
                     refill(s)
 
 
-def iter_windows(model, stores, dataset_config, batch=4, chunk=8, consecutive=None):
+def iter_windows(model, stores, dataset_config, batch=4, chunk=8, consecutive=None, lpips=None):
     """Evaluate the recordings and yield, per model call, a dict of the evaluated windows: "rec" (index into stores), "win"
     (window index), CUDA tensors "esr", "bicubic", "gt" ([n, 2, kH, kW]), "lr" (inp_cnt[mid]), "scaled"
     (inp_scaled_cnt[mid]), "stats" (CUDA float64 [2, n, 2, 6]: metrics.plane_stats of esr and of bicubic against gt) and
-    "events" (the CUDA events around the model call).  Nothing in it synchronises the host with the device.
+    "events" (the CUDA events around the model call); with lpips (an esr_b200.lpips.LPIPS) also "lpips" (CUDA float64
+    [2, n]: esr_lpips and bicubic_lpips).  Nothing in it synchronises the host with the device.
     consecutive: None runs forward_sequence chunks of `chunk` windows when step_size == 1 and the frame-bank path otherwise;
     False forces the frame-bank path (the two give identical outputs; the tests compare them)."""
     check_config(dataset_config)
@@ -199,6 +205,8 @@ def iter_windows(model, stores, dataset_config, batch=4, chunk=8, consecutive=No
                 st["bicubic"] = encodings.interpolate_planes(st["lr"], (kH, kW), "bicubic")
                 n = esr.shape[0]
                 st["stats"] = metrics.plane_stats_device(torch.cat([esr, st["bicubic"]]), torch.cat([st["gt"], st["gt"]])).view(2, n, 2, 6)
+                if lpips is not None:
+                    st["lpips"] = lpips.window_pairs(esr, st["bicubic"], st["gt"])
                 yield st
 
 
@@ -207,12 +215,12 @@ def _save_png(path, arr):
     Image.fromarray(arr).save(path)
 
 
-def evaluate_recordings(model, stores, dataset_config, batch=4, image_dir=None, chunk=8, consecutive=None):
+def evaluate_recordings(model, stores, dataset_config, batch=4, image_dir=None, chunk=8, consecutive=None, lpips=None):
     """infer_ours_cnt.py infer mode 1 over `stores` (EventStore objects, one per recording; named by the file's basename)
     with the dataset config `dataset_config` (dataloader_config['dataset']).  -> (results_dict, results_mean) laid out as
     the script's (:336-347): results_dict[key][name] = the recording's MetricTracker average, results_mean[key] = the mean
-    over recordings, for the keys of METRIC_KEYS (`time` in device milliseconds per window).  chunk, consecutive: as for
-    iter_windows."""
+    over recordings, for the keys of METRIC_KEYS (`time` in device milliseconds per window), and of LPIPS_KEYS when
+    `lpips` (an esr_b200.lpips.LPIPS) is given.  chunk, consecutive: as for iter_windows."""
     params = sum(p.numel() for p in model.parameters()) / 1e6
     names = [os.path.basename(s.path) for s in stores]
     if len(set(names)) != len(names):
@@ -226,7 +234,7 @@ def evaluate_recordings(model, stores, dataset_config, batch=4, image_dir=None, 
                 os.makedirs(os.path.join(image_dir, nm, "event_img", kind), exist_ok=False)
     try:
         steps = []
-        for st in iter_windows(model, stores, dataset_config, batch, chunk, consecutive):
+        for st in iter_windows(model, stores, dataset_config, batch, chunk, consecutive, lpips):
             if pool is not None:
                 imgs = [render.render_event_cnt(t) for t in (st["lr"], st["scaled"], st["bicubic"], st["esr"].round(), st["gt"])]
                 host = [im.cpu().numpy() for im in imgs]
@@ -234,30 +242,35 @@ def evaluate_recordings(model, stores, dataset_config, batch=4, image_dir=None, 
                     for kind, h in zip(IMAGE_KINDS, host):
                         writes.append(pool.submit(_save_png, os.path.join(image_dir, names[r], "event_img", kind, "{:09d}.png".format(w)),
                                                   h[j]))
-            steps.append((st["rec"], st["win"], st["stats"], st["events"], tuple(st["esr"].shape[1:])))
+            steps.append((st["rec"], st["win"], st["stats"], st["events"], tuple(st["esr"].shape[1:]), st.get("lpips")))
         torch.cuda.synchronize()
-        for recs_, wins, stats, ev, shape in steps:
+        for recs_, wins, stats, ev, shape, lp in steps:
             ms = ev[0].elapsed_time(ev[1]) / len(recs_)
             s = stats.cpu()
+            lp = lp.cpu() if lp is not None else None
             for j, (r, w) in enumerate(zip(recs_, wins)):
                 for pre, k in (("esr_", 0), ("bicubic_", 1)):
                     for key, v in metrics.evaluate_from_stats(s[k, j], shape).items():
                         per[r][pre + key].append((w, v))
+                    if lp is not None:
+                        per[r][pre + "lpips"].append((w, float(lp[k, j])))
                 per[r]["time"].append((w, ms))
         for f in writes:
             f.result()
     finally:
         if pool is not None:
             pool.shutdown(wait=True)
-    results_dict, results_mean = {k: {} for k in METRIC_KEYS}, {}
+    keys = METRIC_KEYS + (LPIPS_KEYS if lpips is not None else ())
+    averaged = [k for k in keys if k != "params"]
+    results_dict, results_mean = {k: {} for k in keys}, {}
     for r, nm in enumerate(names):
-        for key in METRIC_KEYS[:-1]:
+        for key in averaged:
             total = 0.0
             vals = [v for _, v in sorted(per[r][key])]     # frame order
             for v in vals:
                 total += v
             results_dict[key][nm] = total / len(vals)
         results_dict["params"][nm] = params
-    for key in METRIC_KEYS:
+    for key in keys:
         results_mean[key] = float(np.mean(list(results_dict[key].values())))
     return results_dict, results_mean

@@ -313,6 +313,31 @@ int esr_metrics_planes(const float *pred, const float *tgt, int n_planes, int H,
                        void *workspace, size_t workspace_bytes, esr_stream_t stream);
 
 /* ---------------------------------------------------------------------------------------------
+ * LPIPS distance (version 0.1, AlexNet backbone, linear heads, spatial=False) of infer_ours_cnt.py:85,90.
+ * Replaces: loss/restore.py:10-39 perceptual_loss.__call__'s per-image work, i.e.
+ * loss/PerceptualSimilarity/models/__init__.py:32-46 PerceptualLoss.forward (normalize: 2x - 1) ->
+ * networks_basic.py:73-101 PNetLin.forward with ScalingLayer (:103-110), pretrained_networks.py:57-95 alexnet (torchvision
+ * alexnet().features up to relu5), normalize_tensor (__init__.py:48-50), NetLinLayer (:113-120) and spatial_average.
+ *  params    : 15 device pointers to fp32 tensors: torchvision's features.{0,3,6,8,10}.{weight,bias} in that order, then the
+ *              v0.1 heads lin{0..4}.model.1.weight ([1,C,1,1]); blob: esr_lpips_param_bytes() bytes.
+ *  workspace : esr_lpips_workspace_bytes(n_img, H, W) bytes (0: the size is too small -- the second max-pool needs H, W >= 31,
+ *              where the reference raises too), owned by the caller, must outlive the plan; the plan is bound to it.
+ *  forward   : planes fp32 [*][H][W]; channel_src int32 [n_img][3] = the plane of each of image i's three input channels (a
+ *              count plane repeated to 3 channels, or three planes of an RGB image); normalize != 0 applies 2x - 1 first.
+ *              out[p] (fp64) = LPIPS(image pair_a[p], image pair_b[p]) for p < n_pairs; n_img, n_pairs <= the plan's n_img;
+ *              indices must be < n_img.  Deterministic, and a pair's value does not depend on the other pairs or images.
+ *              No allocation and no host synchronisation: graph-capturable.
+ * --------------------------------------------------------------------------------------------- */
+typedef void *esr_lpips_t;
+size_t esr_lpips_param_bytes(void);
+int esr_lpips_pack_params(const float *const *params_host_array_of_device_ptrs, void *blob, esr_stream_t stream);
+size_t esr_lpips_workspace_bytes(int n_img, int H, int W);
+int esr_lpips_create(esr_lpips_t *plan, int n_img, int H, int W, const void *blob, void *workspace, size_t workspace_bytes);
+int esr_lpips_destroy(esr_lpips_t plan);
+int esr_lpips_forward(esr_lpips_t plan, const float *planes, const int32_t *channel_src, int n_img, int normalize, int n_pairs,
+                      const int32_t *pair_a, const int32_t *pair_b, double *out, esr_stream_t stream);
+
+/* ---------------------------------------------------------------------------------------------
  * Event-count images of the evaluation script (myutils/vis_events/matplotlib_plot_events.py:125-248, plot_event_cnt with
  * is_save=False) for B images at once.  cnt: fp32 [B, 2, H, W] (0 positive, 1 negative), H * W < 2^24.
  * color_scheme: 0 gray, 1 green_red, 2 blue_red.  out: uint8 [B, H, W, 3] (gray: [B, H, W]); channels in BGR order when
