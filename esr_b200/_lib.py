@@ -60,6 +60,25 @@ SIGNATURES.update({
 })
 
 
+class ConvSmallDesc(ctypes.Structure):
+    """struct esr_conv_small_desc of include/esr_b200.h"""
+    _fields_ = [
+        ("kind", c_int), ("path", c_int), ("in_f32", c_void_p), ("in_", c_void_p), ("in_n_img", c_int), ("in_img", c_void_p),
+        ("H_in", c_int), ("W_in", c_int), ("pad_top", c_int), ("pad_bottom", c_int), ("pad_left", c_int), ("pad_right", c_int),
+        ("w", c_void_p), ("bias", c_void_p), ("w_head", c_void_p), ("b_head", c_void_p), ("n_img", c_int),
+        ("out", c_void_p), ("out_n_img", c_int), ("out_f32", c_void_p),
+        ("crop_top", c_int), ("crop_left", c_int), ("out_H", c_int), ("out_W", c_int),
+        ("agg_feats", c_void_p), ("agg_n_img", c_int), ("agg_att", c_void_p), ("agg_idx", c_void_p), ("agg_N", c_int),
+        ("workspace", c_void_p), ("workspace_bytes", c_size_t),
+    ]
+
+
+SIGNATURES.update({
+    "esr_conv_small_workspace_bytes": (c_size_t, [c_int, c_int]),
+    "esr_conv_small": (c_int, [ctypes.POINTER(ConvSmallDesc), c_void_p]),
+})
+
+
 SIGNATURES.update({
     "esr_net_param_bytes": (c_size_t, []),
     "esr_net_pack_params": (c_int, [c_void_p, c_void_p, c_void_p]),

@@ -271,6 +271,11 @@ int conv_direct(DirectKind kind, const DirectArgs &a, cudaStream_t st)
 {
     // default: warp-level tensor-core variant (mma_conv.cu) where one exists; ESR_DIRECT_FFMA=1 keeps the fp32 FFMA kernels
     static const bool ffma = getenv("ESR_DIRECT_FFMA") != nullptr;
+    return conv_direct_choice(kind, a, ffma, st);
+}
+
+int conv_direct_choice(DirectKind kind, const DirectArgs &a, bool ffma, cudaStream_t st)
+{
     if (!ffma) {
         const int rc = conv_mma(kind, a, st);
         if (rc != ESR_EINVAL) return rc;
@@ -308,4 +313,114 @@ int pack_direct_weight(const float *w, int cout, int cin, float *dst, cudaStream
     return ESR_OK;
 }
 
+// ---- esr_conv_small: one launch of the plan's small-channel / narrow-output layers, kernel family chosen per call
+namespace {
+struct SmallKind {
+    int cin, cout, ntaps, stride;
+    bool ups;
+    int dk;        // DirectKind of paths 0 and 1 (-1: narrow only)
+    int paths;     // bit p: path p runs this kind in the plan
+};
+const SmallKind SMALL_KINDS[] = {
+    {8, 16, 9, 2, false, DK_HEAD_ENC0, 3}, {16, 32, 9, 2, false, DK_ENC1, 3}, {32, 64, 9, 2, false, DK_ENC2, 3},
+    {32, 1, 9, 1, false, DK_ATT32, 7},     {16, 1, 9, 1, false, DK_ATT16, 7}, {32, 16, 9, 1, true, DK_RECON1, 3},
+    {16, 8, 9, 1, true, DK_RECON2, 3},     {8, 2, 9, 1, false, DK_TAIL, 7},   {64, 1, 9, 1, false, -1, 4},
+    {64, 1, 9, 1, false, -1, 4},           {64, 2, 1, 1, false, -1, 4},
+};
+constexpr int N_SMALL_KINDS = (int)(sizeof(SMALL_KINDS) / sizeof(SMALL_KINDS[0]));
+bool small_ok(int kind, int path) { return kind >= 0 && kind < N_SMALL_KINDS && path >= 0 && path <= 2 && (SMALL_KINDS[kind].paths >> path & 1); }
+size_t align256(size_t b) { return (b + 255) / 256 * 256; }
+// the packed weights of the kind's layer (path 0: pack_mma_weight; otherwise fp32 [tap][ci][co], as pack_direct_weight and
+// pack_narrow_weight write it), then for HEAD_ENC0 the head's [9][2][8]
+size_t small_w_bytes(const SmallKind &k, int path)
+{
+    return path == 0 ? mma_weight_bytes(k.cout, k.cin) : sizeof(float) * k.ntaps * k.cin * k.cout;
+}
+} // namespace
+
 } // namespace esr
+
+using namespace esr;
+
+extern "C" size_t esr_conv_small_workspace_bytes(int kind, int path)
+{
+    if (!small_ok(kind, path)) return 0;
+    return align256(small_w_bytes(SMALL_KINDS[kind], path)) + (kind == ESR_CONV_SMALL_HEAD_ENC0 ? align256(sizeof(float) * 9 * 2 * 8) : 0);
+}
+
+extern "C" int esr_conv_small(const esr_conv_small_desc *d, esr_stream_t stream)
+{
+    ESR_REQUIRE(d, "esr_conv_small: null descriptor");
+    if (!small_ok(d->kind, d->path)) {
+        set_error("esr_conv_small: kind %d has no path %d in the network", d->kind, d->path);
+        return ESR_EUNSUPPORTED;
+    }
+    const SmallKind &k = SMALL_KINDS[d->kind];
+    const bool head = d->kind == ESR_CONV_SMALL_HEAD_ENC0, tail = d->kind == ESR_CONV_SMALL_TAIL;
+    const bool split_out = k.cout >= 8;
+    ESR_REQUIRE(d->n_img > 0 && d->H_in > 0 && d->W_in > 0, "esr_conv_small: n_img=%d H_in=%d W_in=%d", d->n_img, d->H_in, d->W_in);
+    ESR_REQUIRE(d->workspace && d->workspace_bytes >= esr_conv_small_workspace_bytes(d->kind, d->path), "esr_conv_small: workspace");
+    ESR_REQUIRE(d->w && d->bias && (head ? d->in_f32 && d->w_head && d->b_head : d->in && d->in_n_img > 0),
+                "esr_conv_small: missing input or weights");
+    ESR_REQUIRE(split_out ? d->out && d->out_n_img >= d->n_img : d->out_f32 != nullptr, "esr_conv_small: missing output");
+    ESR_REQUIRE(head || (d->pad_top | d->pad_bottom | d->pad_left | d->pad_right) == 0, "esr_conv_small: pads are HEAD_ENC0's");
+    ESR_REQUIRE(d->pad_top >= 0 && d->pad_bottom >= 0 && d->pad_left >= 0 && d->pad_right >= 0, "esr_conv_small: negative pad");
+    if (d->agg_feats && (d->path != 0 || !k.ups)) {
+        set_error("esr_conv_small: scale aggregation is fused into the mma decoder kernels only");
+        return ESR_EUNSUPPORTED;
+    }
+    ESR_REQUIRE(!d->agg_feats || (d->agg_att && d->agg_N > 0 && d->agg_n_img > 0), "esr_conv_small: agg_att / agg_N / agg_n_img");
+    if (tail && d->path == 2 && d->in_img) {
+        set_error("esr_conv_small: the narrow tail kernel reads images in order");
+        return ESR_EUNSUPPORTED;
+    }
+    const int Hc = d->H_in + d->pad_top + d->pad_bottom, Wc = d->W_in + d->pad_left + d->pad_right;
+    const int Hout = k.ups ? 2 * Hc : (k.stride == 2 ? (Hc - 1) / 2 + 1 : Hc);
+    const int Wout = k.ups ? 2 * Wc : (k.stride == 2 ? (Wc - 1) / 2 + 1 : Wc);
+    ESR_REQUIRE(!tail || (d->crop_top >= 0 && d->crop_left >= 0 && d->out_H > 0 && d->out_W > 0 && d->crop_top + d->out_H <= Hout &&
+                          d->crop_left + d->out_W <= Wout),
+                "esr_conv_small: crop window (%d, %d) %d x %d outside %d x %d", d->crop_top, d->crop_left, d->out_H, d->out_W, Hout, Wout);
+
+    cudaStream_t st = (cudaStream_t)stream;
+    uint8_t *ws = (uint8_t *)d->workspace;
+    int rc;
+    if (d->path == 0) rc = pack_mma_weight(d->w, k.cout, k.cin, ws, st);
+    else if (k.cin == 64) rc = pack_narrow_weight(d->w, k.cout, k.ntaps, (float *)ws, st);
+    else rc = pack_direct_weight(d->w, k.cout, k.cin, (float *)ws, st);
+    if (rc) return rc;
+    float *w_head = (float *)(ws + align256(small_w_bytes(k, d->path)));
+    if (head && (rc = pack_direct_weight(d->w_head, 8, 2, w_head, st))) return rc;
+
+    const size_t in_plane = (size_t)d->in_n_img * d->H_in * d->W_in * k.cin;
+    if (d->path == 2) {
+        SplitTensor x;
+        x.base = (__nv_bfloat16 *)d->in; x.n_img = d->in_n_img; x.H = d->H_in; x.W = d->W_in; x.C = k.cin;
+        if (tail) return conv_narrow_tail(x, (const float *)ws, d->bias, d->n_img, d->out_f32, d->crop_top, d->crop_left, d->out_H, d->out_W, st);
+        return conv_narrow(x, d->in_img, (const float *)ws, d->bias, k.cout, k.ntaps, d->n_img, d->out_f32, st);
+    }
+    DirectArgs a;
+    a.in_img = d->in_img; a.Hin = d->H_in; a.Win = d->W_in;
+    a.w = (const float *)ws; a.w_mma = ws; a.bias = d->bias;
+    a.act = k.cout == 1 ? ACT_SIGMOID : ACT_RELU;
+    a.n_img = d->n_img; a.Hout = Hout; a.Wout = Wout;
+    if (head) {
+        a.in_f32 = d->in_f32; a.w0 = w_head; a.b0 = d->b_head;
+        a.pad_top = d->pad_top; a.pad_bottom = d->pad_bottom; a.pad_left = d->pad_left; a.pad_right = d->pad_right;
+    } else {
+        a.in_split = (const __nv_bfloat16 *)d->in; a.in_plane = in_plane;
+    }
+    if (split_out) {
+        a.out_split = (__nv_bfloat16 *)d->out; a.out_plane = (size_t)d->out_n_img * Hout * Wout * k.cout;
+    } else {
+        a.out_f32 = d->out_f32;
+        if (tail) { a.crop_top = d->crop_top; a.crop_left = d->crop_left; a.out_H = d->out_H; a.out_W = d->out_W; }
+    }
+    if (d->agg_feats) {
+        a.agg_feats = (const __nv_bfloat16 *)d->agg_feats; a.agg_plane = (size_t)d->agg_n_img * d->H_in * d->W_in * k.cin;
+        a.agg_att = d->agg_att; a.agg_idx = d->agg_idx; a.agg_N = d->agg_N;
+    }
+    if (d->path == 1) return conv_direct_choice((DirectKind)k.dk, a, true, st);
+    rc = conv_mma((DirectKind)k.dk, a, st);
+    if (rc == ESR_EINVAL) set_error("esr_conv_small: kind %d has no mma instantiation", d->kind);
+    return rc;
+}

@@ -34,6 +34,8 @@ struct DirectArgs {
 };
 
 int conv_direct(DirectKind kind, const DirectArgs &a, cudaStream_t st);
+// conv_direct with the kernel family chosen by the caller (ffma: the fp32 FFMA kernels even where an mma variant exists)
+int conv_direct_choice(DirectKind kind, const DirectArgs &a, bool ffma, cudaStream_t st);
 // mma_conv.cu: the same layers on mma.sync tensor cores; ESR_EINVAL = this kind has no mma variant (use the FFMA kernel)
 int conv_mma(DirectKind kind, const DirectArgs &a, cudaStream_t st);
 int pack_direct_weight(const float *w, int cout, int cin, float *dst, cudaStream_t st);

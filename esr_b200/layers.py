@@ -97,3 +97,63 @@ def conv_tc(srcs, wpacked, bias, cout, ntaps=9, act=None, act_from=0, src_img=No
         _lib.check(_lib.lib().esr_conv_tc_chunked(ctypes.byref(d), chunks, steps, _lib.stream_ptr()), "esr_conv_tc_chunked")
     torch.cuda.current_stream().synchronize() if keep else None
     return out, out_f32
+
+
+# esr_conv_small kinds (include/esr_b200.h) and paths
+SMALL_KINDS = {"head_enc0": 0, "enc1": 1, "enc2": 2, "att32": 3, "att16": 4, "recon1": 5, "recon2": 6, "tail": 7,
+               "pred_map1": 8, "atten0": 9, "spatial_kernel": 10}
+SMALL_PATHS = {"mma": 0, "ffma": 1, "narrow": 2}
+
+
+def conv_small_supported(kind, path):
+    return _lib.lib().esr_conv_small_workspace_bytes(SMALL_KINDS[kind], SMALL_PATHS[path]) > 0
+
+
+def conv_small(kind, path, x, w, bias, n_img, out=None, out_f32=None, in_img=None, pads=(0, 0, 0, 0), head=None,
+               crop=None, agg=None):
+    """One small-channel / narrow-output layer of the network (esr_conv_small) on kernel family `path`.
+    x: Split, or fp32 NCHW [*, 2, H, W] for head_enc0 (then head = (w_head, b_head), pads = (top, bottom, left, right));
+    out: Split for Cout >= 8, else out_f32 (NHWC, or NCHW [n_img, 2, out_H, out_W] with crop = (top, left) for the tail);
+    agg = (feats Split, att fp32 [feats.n_img, H, W], idx int [n_img * N] or None, N) for recon1 / recon2."""
+    L = _lib.lib()
+    k, p = SMALL_KINDS[kind], SMALL_PATHS[path]
+    d = _lib.ConvSmallDesc()
+    d.kind, d.path, d.n_img = k, p, n_img
+    w, bias = w.contiguous().float(), bias.contiguous().float()
+    keep = []
+
+    def dev_i32(t):
+        t = t.to(device=w.device, dtype=torch.int32).contiguous()
+        keep.append(t)
+        return t.data_ptr()
+
+    if kind == "head_enc0":
+        x = x.contiguous()
+        keep.append(x)
+        d.in_f32, d.in_n_img, d.H_in, d.W_in = x.data_ptr(), x.shape[0], x.shape[2], x.shape[3]
+        d.pad_top, d.pad_bottom, d.pad_left, d.pad_right = pads
+        head = [t.contiguous().float() for t in head]
+        d.w_head, d.b_head = head[0].data_ptr(), head[1].data_ptr()
+    else:
+        d.in_, d.in_n_img, d.H_in, d.W_in = x.buf.data_ptr(), x.n_img, x.H, x.W
+    if in_img is not None:
+        d.in_img = dev_i32(in_img)
+    d.w, d.bias = w.data_ptr(), bias.data_ptr()
+    if out is not None:
+        d.out, d.out_n_img = out.buf.data_ptr(), out.n_img
+    if out_f32 is not None:
+        d.out_f32 = out_f32.data_ptr()
+        if crop is not None:
+            d.crop_top, d.crop_left = crop
+            d.out_H, d.out_W = out_f32.shape[2], out_f32.shape[3]
+    if agg is not None:
+        feats, att, idx, N = agg
+        d.agg_feats, d.agg_n_img, d.agg_att, d.agg_N = feats.buf.data_ptr(), feats.n_img, att.data_ptr(), N
+        if idx is not None:
+            d.agg_idx = dev_i32(idx)
+    nbytes = L.esr_conv_small_workspace_bytes(k, p)
+    ws = torch.empty((max(nbytes, 1),), dtype=torch.uint8, device=w.device)
+    d.workspace, d.workspace_bytes = ws.data_ptr(), nbytes
+    _lib.check(L.esr_conv_small(ctypes.byref(d), _lib.stream_ptr()), f"esr_conv_small({kind}, {path})")
+    torch.cuda.current_stream().synchronize()
+    return out if out is not None else out_f32

@@ -163,6 +163,51 @@ int esr_split_from_nchw(const float *src, int n_img, int C, int H, int W, void *
 int esr_split_to_nchw(const void *src, int n_img, int C, int H, int W, float *dst, esr_stream_t stream);
 
 /* ---------------------------------------------------------------------------------------------
+ * Small-channel and narrow-output convolutions, layer by layer (for tests and tools; the network launches the same kernels
+ * from esr_net_forward).  One call runs one launch of the network's plan on a chosen kernel family:
+ *   path 0 = warp-level tensor cores (mma.sync, split bf16), 1 = fp32 FFMA twins, 2 = the narrow-output CUDA-core kernels.
+ * A (kind, path) pair the network never runs returns ESR_EUNSUPPORTED.
+ *   kind             Cin -> Cout, stride, act; input; output                                       paths
+ *   HEAD_ENC0        2 -> 8 relu (head, w_head / b_head) fused into 8 -> 16 stride 2 relu; fp32 NCHW [*, 2, H_in, W_in]
+ *                    zero-padded by pad_* (CropSize); split out                                    0, 1
+ *   ENC1 / ENC2      16 -> 32 / 32 -> 64, stride 2, relu; split in and out                         0, 1
+ *   ATT32 / ATT16    32 -> 1 / 16 -> 1, sigmoid; split in; fp32 NHWC out [n_img, H_in, W_in, 1]    0, 1, 2
+ *   RECON1 / RECON2  bilinear x2, then 32 -> 16 / 16 -> 8 relu; split in and out (2 H_in x 2 W_in);
+ *                    agg_feats != NULL (path 0): the source is in + mean over n < agg_N of
+ *                    agg_feats[agg_idx[img * agg_N + n]] * agg_att[same image and pixel]          0, 1
+ *   TAIL             8 -> 2 relu; split in; fp32 NCHW out [n_img, 2, out_H, out_W] = the window at (crop_top, crop_left)
+ *                    of the H_in x W_in result                                                     0, 1, 2
+ *   PRED_MAP1 / ATTEN0  64 -> 1, 3x3, sigmoid; SPATIAL_KERNEL 64 -> 2, 1x1, sigmoid; split in; fp32 NHWC out   2
+ * Weights are fp32 [Cout, Cin, k, k], packed into `workspace` (esr_conv_small_workspace_bytes(kind, path) bytes) on `stream` by
+ * the network's own packers.  Split tensors are [2 planes][n_img][H][W][C] bf16; in_n_img / out_n_img / agg_n_img give the
+ * images per plane.  in_img (optional, not with TAIL on path 2): output image -> input image.  Stride-2 outputs are
+ * (H - 1) / 2 + 1 high for a conv input of H rows (H_in + pad_top + pad_bottom for HEAD_ENC0).
+ * --------------------------------------------------------------------------------------------- */
+enum {
+    ESR_CONV_SMALL_HEAD_ENC0 = 0, ESR_CONV_SMALL_ENC1, ESR_CONV_SMALL_ENC2, ESR_CONV_SMALL_ATT32, ESR_CONV_SMALL_ATT16,
+    ESR_CONV_SMALL_RECON1, ESR_CONV_SMALL_RECON2, ESR_CONV_SMALL_TAIL, ESR_CONV_SMALL_PRED_MAP1, ESR_CONV_SMALL_ATTEN0,
+    ESR_CONV_SMALL_SPATIAL_KERNEL
+};
+typedef struct esr_conv_small_desc {
+    int kind, path;
+    const float *in_f32;                    /* HEAD_ENC0 */
+    const void *in; int in_n_img;           /* the other kinds */
+    const int32_t *in_img;
+    int H_in, W_in;
+    int pad_top, pad_bottom, pad_left, pad_right;   /* HEAD_ENC0 */
+    const float *w, *bias;
+    const float *w_head, *b_head;           /* HEAD_ENC0: [8, 2, 3, 3], [8] */
+    int n_img;
+    void *out; int out_n_img;               /* split output */
+    float *out_f32;                         /* fp32 output */
+    int crop_top, crop_left, out_H, out_W;  /* TAIL */
+    const void *agg_feats; int agg_n_img; const float *agg_att; const int32_t *agg_idx; int agg_N;   /* RECON1 / RECON2 */
+    void *workspace; size_t workspace_bytes;
+} esr_conv_small_desc;
+size_t esr_conv_small_workspace_bytes(int kind, int path);
+int esr_conv_small(const esr_conv_small_desc *desc, esr_stream_t stream);
+
+/* ---------------------------------------------------------------------------------------------
  * The network: DeepRecurrNet.forward with carried ConvGRU states.
  * Replaces: models/model.py:294-344 (DeepRecurrNet.forward / reset_states), and underneath it
  * models/model.py:20-291, models/submodules.py (ConvLayer, UpsampleConvLayer, ResidualBlock, RecurrentConvLayer,

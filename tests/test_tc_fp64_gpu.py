@@ -127,11 +127,12 @@ TOL = {
 }
 
 
-def check(name, kind, got, ref, degraded, degraded_is="A_lo B_hi dropped"):
-    """err <= TOL[kind] and TOL[kind] <= err(degraded) / 4 (degraded None: no product term to lose)."""
+def check(name, kind, got, ref, degraded, degraded_is="A_lo B_hi dropped", tol=None):
+    """err <= TOL[kind] and TOL[kind] <= err(degraded) / 4 (degraded None: no product term to lose).  tol: the
+    tolerance of a kind another test module defines."""
     err = rel(got, ref)
     deg = rel(degraded, ref) if degraded is not None else None
-    tol = TOL[kind]
+    tol = TOL[kind] if tol is None else tol
     print(f"[tc64] {name} [{kind}]: err {err:.2e}, TOL {tol:.1e}, degraded {'n/a' if deg is None else format(deg, '.2e')}"
           f"{'' if deg is None else ' (' + degraded_is + ')'}")
     assert err <= tol, (name, kind, err, tol)
