@@ -137,6 +137,17 @@ SIGNATURES.update({
     "esr_adam_step_dev": (c_int, [c_void_p] * 5 + [c_size_t, c_void_p, c_void_p, c_void_p]),
 })
 
+# the *_ex training entry points: a `flags` word before the workspace (DETERMINISTIC = ESR_DETERMINISTIC of the header)
+DETERMINISTIC = 1
+SIGNATURES.update({
+    "esr_conv2d_workspace_bytes_ex": (c_size_t, [c_int] * 8),
+    "esr_conv2d_backward_ex": (c_int, [c_void_p] * 5 + [c_int] * 8 + [c_void_p] * 3 + [c_int, c_void_p, c_size_t, c_void_p]),
+    "esr_dcn_v2_backward_workspace_bytes_ex": (c_size_t, [c_int] * 11),
+    "esr_dcn_v2_backward_ex": (c_int, [c_void_p] * 6 + [c_int] * 10 + [c_void_p] * 5 + [c_int, c_void_p, c_size_t, c_void_p]),
+    "esr_mse_loss_workspace_bytes_ex": (c_size_t, [c_size_t, c_int]),
+    "esr_mse_loss_ex": (c_int, [c_void_p, c_void_p, c_size_t, c_void_p, c_void_p, c_float, c_int, c_void_p, c_size_t, c_void_p]),
+})
+
 
 class ESRError(RuntimeError):
     pass

@@ -9,6 +9,8 @@
 //   3. grad_weight[co][c][tap] = sum_p gO[p][co] * cols[p][tap*64+c]   (cols re-sampled by dcn_columns; tiled fp32 GEMM
 //      over pixel slices with atomicAdd of the partial tiles),  grad_bias[co] = sum_p gO[p][co].
 // Configuration: the one ESR uses (64 -> 64, 3x3, stride 1, pad 1, dilation 1, 8 deformable groups).
+// Deterministic mode (ESR_DETERMINISTIC, esr_dcn_v2_backward_ex): grad_input in int64 fixed point, grad_weight / grad_bias from
+// per-slice partials added in slice order -- bitwise reproducible.
 #include "net.cuh"
 
 namespace esr {
@@ -34,11 +36,46 @@ __global__ void k_dcn_wt(const float *__restrict__ w, float *__restrict__ wt)
     wt[i] = w[((size_t)co * 64 + c) * 9 + tap];
 }
 
-// offset/mask NCHW -> om NHWC [p][216] is k_om_from_nchw in dcn.cu; grads go back the other way
+// ---- deterministic grad_input (ESR_DETERMINISTIC): the bilinear scatter's targets depend on the learned offsets, so instead of
+// fp32 atomics it accumulates in int64 fixed point, whose atomics give the same sum in any order.  A pre-pass takes the largest
+// |gcols * mask| over the batch (order-independent max); every scattered value is that product times a corner weight <= 1.
+// The scale is the power of two that keeps the worst case -- all 72 (tap, group) x 4 corner values of every pixel of an image
+// landing on one element, each rounded up by half a unit -- below 2^63: 288 * H * W * (max * scale + 1/2) <= 2^62 + 144 H W.
+__device__ __forceinline__ double dcn_fixed_scale(unsigned max_bits, int H, int W)
+{
+    const float m = __uint_as_float(max_bits);
+    if (!(m > 0.0f)) return 1.0;
+    return exp2(floor(log2(0x1p62 / (288.0 * (double)H * (double)W * (double)m))));
+}
+
+// max over (p, tap, group, channel) of |gcols * mask|: thread per (p, tap, group), warp max, one atomicMax per warp on the bit
+// pattern (the values are >= 0, so the unsigned order of the bits is the float order)
 __global__ void __launch_bounds__(256)
-k_dcn_bwd_sample(const __nv_bfloat16 *__restrict__ feat, size_t f_plane, const float *__restrict__ om,
-                 const float *__restrict__ gcols, int n_img, int H, int W, float *__restrict__ gin /*[p][64]*/,
-                 float *__restrict__ gom /*[p][216]*/)
+k_dcn_gin_max(const float *__restrict__ om, const float *__restrict__ gcols, size_t total, unsigned *__restrict__ max_bits)
+{
+    unsigned mx = 0u;
+    for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
+        const int g = (int)(i % 8), k = (int)((i / 8) % 9);
+        const size_t p = i / 72;
+        const float m = om[p * 216 + 144 + g * 9 + k];
+        const float4 *gp = reinterpret_cast<const float4 *>(gcols + p * 576 + k * 64 + g * 8);
+        const float4 ga = gp[0], gb = gp[1];
+        const float gc[8] = {ga.x, ga.y, ga.z, ga.w, gb.x, gb.y, gb.z, gb.w};
+#pragma unroll
+        for (int e = 0; e < 8; ++e) mx = max(mx, __float_as_uint(fabsf(gc[e] * m)));
+    }
+    mx = __reduce_max_sync(0xffffffffu, mx);
+    if ((threadIdx.x & 31) == 0 && mx) atomicMax(max_bits, mx);
+}
+
+__device__ __forceinline__ unsigned long long to_fixed(float v, double scale) { return (unsigned long long)__double2ll_rn((double)v * scale); }
+
+// offset/mask NCHW -> om NHWC [p][216] is k_om_from_nchw in dcn.cu; grads go back the other way
+// DET: grad_input goes to gin_q (int64 fixed point at `scale`) instead of gin
+template <bool DET>
+__device__ __forceinline__ void dcn_bwd_sample_body(const __nv_bfloat16 *__restrict__ feat, size_t f_plane, const float *__restrict__ om,
+                                                    const float *__restrict__ gcols, int n_img, int H, int W, float *__restrict__ gin,
+                                                    unsigned long long *__restrict__ gin_q, double scale, float *__restrict__ gom)
 {
     const size_t total = (size_t)n_img * H * W * 72;
     for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
@@ -78,10 +115,17 @@ k_dcn_bwd_sample(const __nv_bfloat16 *__restrict__ feat, size_t f_plane, const f
                 g_off_h += gc[e] * m * (hw * (c3[e] - c1[e]) + lw * (c4[e] - c2[e]));
                 g_off_w += gc[e] * m * (hh * (c2[e] - c1[e]) + lh * (c4[e] - c3[e]));
                 const float t = gc[e] * m;
-                if (ok1) atomicAdd(gin + p1 * 64 + g * 8 + e, w1 * t);
-                if (ok2) atomicAdd(gin + p2 * 64 + g * 8 + e, w2 * t);
-                if (ok3) atomicAdd(gin + p3 * 64 + g * 8 + e, w3 * t);
-                if (ok4) atomicAdd(gin + p4 * 64 + g * 8 + e, w4 * t);
+                if (DET) {
+                    if (ok1) atomicAdd(gin_q + p1 * 64 + g * 8 + e, to_fixed(w1 * t, scale));
+                    if (ok2) atomicAdd(gin_q + p2 * 64 + g * 8 + e, to_fixed(w2 * t, scale));
+                    if (ok3) atomicAdd(gin_q + p3 * 64 + g * 8 + e, to_fixed(w3 * t, scale));
+                    if (ok4) atomicAdd(gin_q + p4 * 64 + g * 8 + e, to_fixed(w4 * t, scale));
+                } else {
+                    if (ok1) atomicAdd(gin + p1 * 64 + g * 8 + e, w1 * t);
+                    if (ok2) atomicAdd(gin + p2 * 64 + g * 8 + e, w2 * t);
+                    if (ok3) atomicAdd(gin + p3 * 64 + g * 8 + e, w3 * t);
+                    if (ok4) atomicAdd(gin + p4 * 64 + g * 8 + e, w4 * t);
+                }
             }
         }
         float *go = gom + p * 216;
@@ -90,12 +134,38 @@ k_dcn_bwd_sample(const __nv_bfloat16 *__restrict__ feat, size_t f_plane, const f
         go[144 + g * 9 + k] = g_mask;
     }
 }
-
-// grad_weight partial tiles: block = 64 co x 64 columns (one tap), over a slice of PSL pixels
-constexpr int WG_PSL = 512;
 __global__ void __launch_bounds__(256)
-k_dcn_wgrad(const float *__restrict__ go /*[p][64] fp32 NHWC*/, const __nv_bfloat16 *__restrict__ cols, size_t c_plane,
-            size_t npix, float *__restrict__ gw /*[co][c][tap]*/)
+k_dcn_bwd_sample(const __nv_bfloat16 *__restrict__ feat, size_t f_plane, const float *__restrict__ om,
+                 const float *__restrict__ gcols, int n_img, int H, int W, float *__restrict__ gin /*[p][64]*/,
+                 float *__restrict__ gom /*[p][216]*/)
+{
+    dcn_bwd_sample_body<false>(feat, f_plane, om, gcols, n_img, H, W, gin, nullptr, 0.0, gom);
+}
+__global__ void __launch_bounds__(256)
+k_dcn_bwd_sample_det(const __nv_bfloat16 *__restrict__ feat, size_t f_plane, const float *__restrict__ om,
+                     const float *__restrict__ gcols, int n_img, int H, int W, const unsigned *__restrict__ max_bits,
+                     unsigned long long *__restrict__ gin_q /*[p][64]*/, float *__restrict__ gom /*[p][216]*/)
+{
+    dcn_bwd_sample_body<true>(feat, f_plane, om, gcols, n_img, H, W, nullptr, gin_q, dcn_fixed_scale(*max_bits, H, W), gom);
+}
+
+// fixed-point grad_input [p][64] -> fp32 NCHW
+__global__ void k_dcn_gin_from_fixed(const long long *__restrict__ q, const unsigned *__restrict__ max_bits, int n_img, int HW,
+                                     float *__restrict__ dst)
+{
+    const double inv = 1.0 / dcn_fixed_scale(*max_bits, 1, HW);
+    const size_t total = (size_t)n_img * 64 * HW;
+    for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
+        const int pix = (int)(i % HW), c = (int)((i / HW) % 64), n = (int)(i / ((size_t)HW * 64));
+        dst[i] = (float)((double)q[((size_t)n * HW + pix) * 64 + c] * inv);
+    }
+}
+
+// grad_weight partial tiles: block = 64 co x 64 columns (one tap), over a slice of PSL pixels.  DET: slice y -> gw[y][co][c][tap]
+constexpr int WG_PSL = 512;
+template <bool DET>
+__device__ __forceinline__ void dcn_wgrad_body(const float *__restrict__ go, const __nv_bfloat16 *__restrict__ cols, size_t c_plane,
+                                               size_t npix, float *__restrict__ gw)
 {
     __shared__ float sA[32][65];   // gO[pix][co]
     __shared__ float sB[32][65];   // cols[pix][c] of this tap
@@ -136,15 +206,41 @@ k_dcn_wgrad(const float *__restrict__ go /*[p][64] fp32 NHWC*/, const __nv_bfloa
 #pragma unroll
     for (int i = 0; i < 4; ++i)
 #pragma unroll
-        for (int j = 0; j < 4; ++j) atomicAdd(gw + ((size_t)(ty * 4 + i) * 64 + tx * 4 + j) * 9 + tap, acc[i][j]);
+        for (int j = 0; j < 4; ++j) {
+            if (DET) gw[(size_t)blockIdx.y * 64 * 64 * 9 + ((size_t)(ty * 4 + i) * 64 + tx * 4 + j) * 9 + tap] = acc[i][j];
+            else atomicAdd(gw + ((size_t)(ty * 4 + i) * 64 + tx * 4 + j) * 9 + tap, acc[i][j]);
+        }
+}
+__global__ void __launch_bounds__(256)
+k_dcn_wgrad(const float *__restrict__ go /*[p][64] fp32 NHWC*/, const __nv_bfloat16 *__restrict__ cols, size_t c_plane,
+            size_t npix, float *__restrict__ gw /*[co][c][tap]*/)
+{
+    dcn_wgrad_body<false>(go, cols, c_plane, npix, gw);
+}
+__global__ void __launch_bounds__(256)
+k_dcn_wgrad_det(const float *__restrict__ go, const __nv_bfloat16 *__restrict__ cols, size_t c_plane, size_t npix, float *__restrict__ part)
+{
+    dcn_wgrad_body<true>(go, cols, c_plane, npix, part);
 }
 
-__global__ void __launch_bounds__(256) k_dcn_bgrad(const float *__restrict__ go, size_t npix, float *__restrict__ gb)
+// DET: thread (block b, lane_p) -> gb[b * 4 + lane_p][co]
+constexpr int BG_BLOCKS = 148;
+template <bool DET>
+__device__ __forceinline__ void dcn_bgrad_body(const float *__restrict__ go, size_t npix, float *__restrict__ gb)
 {
     const int co = threadIdx.x % 64, lane_p = threadIdx.x / 64;
     float s = 0.0f;
     for (size_t p = (size_t)blockIdx.x * 4 + lane_p; p < npix; p += (size_t)gridDim.x * 4) s += go[p * 64 + co];
-    atomicAdd(gb + co, s);
+    if (DET) gb[((size_t)blockIdx.x * 4 + lane_p) * 64 + co] = s;
+    else atomicAdd(gb + co, s);
+}
+__global__ void __launch_bounds__(256) k_dcn_bgrad(const float *__restrict__ go, size_t npix, float *__restrict__ gb)
+{
+    dcn_bgrad_body<false>(go, npix, gb);
+}
+__global__ void __launch_bounds__(256) k_dcn_bgrad_det(const float *__restrict__ go, size_t npix, float *__restrict__ part)
+{
+    dcn_bgrad_body<true>(go, npix, part);
 }
 
 // NCHW fp32 <-> NHWC fp32 helpers
@@ -172,21 +268,35 @@ __global__ void k_nhwc_to_nchw(const float *__restrict__ src, int n_img, int C, 
 
 using namespace esr;
 
-struct DcnBwdWs { size_t feat, om, go_split, go_nhwc, gcols, cols, gin, gom, wt, wtp, bz, total; };
-static DcnBwdWs dcn_bwd_layout(int B, int H, int W)
+// det: grad_input in int64 fixed point (twice the bytes), then the partial buffers of grad_weight / grad_bias and the max word
+struct DcnBwdWs { size_t feat, om, go_split, go_nhwc, gcols, cols, gin, gom, wt, wtp, bz, wpart, bpart, maxw, total; };
+static DcnBwdWs dcn_bwd_layout(int B, int H, int W, bool det)
 {
     DcnBwdWs l{};
     size_t off = 0;
     auto take = [&](size_t bytes) { size_t r = off; off = align_up(off + bytes, 1024); return r; };
     const size_t px = (size_t)B * H * W;
     l.feat = take(px * 64 * 4); l.om = take(px * 216 * 4); l.go_split = take(px * 64 * 4); l.go_nhwc = take(px * 64 * 4);
-    l.gcols = take(px * 576 * 4); l.cols = take(px * 576 * 4); l.gin = take(px * 64 * 4); l.gom = take(px * 216 * 4);
+    l.gcols = take(px * 576 * 4); l.cols = take(px * 576 * 4); l.gin = take(px * 64 * (det ? 8 : 4)); l.gom = take(px * 216 * 4);
     l.wt = take(576 * 64 * 4); l.wtp = take(3 * tc_packed_weight_bytes(192, 64, 1)); l.bz = take(256 * 4);
+    if (det) {
+        l.wpart = take((size_t)ceil_div64((int64_t)px, WG_PSL) * 64 * 64 * 9 * 4);
+        l.bpart = take((size_t)BG_BLOCKS * 4 * 64 * 4);
+        l.maxw = take(4);
+    }
     l.total = off;
     return l;
 }
 
-extern "C" size_t esr_dcn_v2_backward_workspace_bytes(int B, int H, int W) { return dcn_bwd_layout(B, H, W).total; }
+extern "C" size_t esr_dcn_v2_backward_workspace_bytes(int B, int H, int W) { return dcn_bwd_layout(B, H, W, false).total; }
+
+extern "C" size_t esr_dcn_v2_backward_workspace_bytes_ex(int B, int C, int H, int W, int Co, int kernel, int stride, int pad,
+                                                         int dilation, int deformable_group, int flags)
+{
+    if (dcn_is_tuned(C, Co, kernel, stride, pad, dilation, deformable_group))
+        return dcn_bwd_layout(B, H, W, (flags & ESR_DETERMINISTIC) != 0).total;
+    return dcn_generic_ws_bytes(B, C, H, W, Co, kernel, stride, pad, dilation, deformable_group, 1);
+}
 
 extern "C" int esr_dcn_v2_backward(const float *input, const float *weight, const float *bias, const float *offset,
                                    const float *mask, const float *grad_output, int B, int C, int H, int W, int Co, int kernel,
@@ -194,14 +304,33 @@ extern "C" int esr_dcn_v2_backward(const float *input, const float *weight, cons
                                    float *grad_offset, float *grad_mask, float *grad_weight, float *grad_bias, void *workspace,
                                    size_t ws_bytes, esr_stream_t stream)
 {
+    return esr_dcn_v2_backward_ex(input, weight, bias, offset, mask, grad_output, B, C, H, W, Co, kernel, stride, pad, dilation,
+                                  deformable_group, grad_input, grad_offset, grad_mask, grad_weight, grad_bias, 0, workspace, ws_bytes,
+                                  stream);
+}
+
+extern "C" int esr_dcn_v2_backward_ex(const float *input, const float *weight, const float *bias, const float *offset,
+                                      const float *mask, const float *grad_output, int B, int C, int H, int W, int Co, int kernel,
+                                      int stride, int pad, int dilation, int deformable_group, float *grad_input,
+                                      float *grad_offset, float *grad_mask, float *grad_weight, float *grad_bias, int flags,
+                                      void *workspace, size_t ws_bytes, esr_stream_t stream)
+{
     (void)bias;
     ESR_REQUIRE(input && weight && offset && mask && grad_output && grad_input && grad_offset && grad_mask && grad_weight &&
                 grad_bias && workspace, "esr_dcn_v2_backward: null pointer");
-    if (!dcn_is_tuned(C, Co, kernel, stride, pad, dilation, deformable_group))      // any other configuration: dcn_generic.cu
+    const bool det = (flags & ESR_DETERMINISTIC) != 0;
+    if (!dcn_is_tuned(C, Co, kernel, stride, pad, dilation, deformable_group)) {    // any other configuration: dcn_generic.cu
+        if (det) {
+            set_error("esr_dcn_v2_backward: only the 64 -> 64, 3x3, stride 1, pad 1, dilation 1, 8-group configuration has a "
+                      "deterministic backward (this is C=%d Co=%d k=%d s=%d p=%d d=%d dg=%d); leave deterministic mode for it",
+                      C, Co, kernel, stride, pad, dilation, deformable_group);
+            return ESR_EUNSUPPORTED;
+        }
         return dcn_generic_backward(input, weight, offset, mask, grad_output, B, C, H, W, Co, kernel, stride, pad, dilation,
                                     deformable_group, grad_input, grad_offset, grad_mask, grad_weight, grad_bias, workspace, ws_bytes,
                                     (cudaStream_t)stream);
-    const DcnBwdWs L = dcn_bwd_layout(B, H, W);
+    }
+    const DcnBwdWs L = dcn_bwd_layout(B, H, W, det);
     if (ws_bytes < L.total) { set_error("esr_dcn_v2_backward: workspace %zu < %zu", ws_bytes, L.total); return ESR_EWORKSPACE; }
     cudaStream_t st = (cudaStream_t)stream;
     char *ws = (char *)workspace;
@@ -221,7 +350,7 @@ extern "C" int esr_dcn_v2_backward(const float *input, const float *weight, cons
     ESR_LAUNCH_CHECK();
     if ((rc = om_from_nchw(offset, mask, B, HW, om, st))) return rc;
     ESR_CUDA_CHECK(cudaMemsetAsync(bz, 0, 256 * 4, st));
-    ESR_CUDA_CHECK(cudaMemsetAsync(gin, 0, px * 64 * 4, st));
+    ESR_CUDA_CHECK(cudaMemsetAsync(gin, 0, px * 64 * (det ? 8 : 4), st));
     ESR_CUDA_CHECK(cudaMemsetAsync(grad_weight, 0, 64 * 64 * 9 * 4, st));
     ESR_CUDA_CHECK(cudaMemsetAsync(grad_bias, 0, 64 * 4, st));
     // 1. gcols = gO . W^T  (three N=192 slices of the 576 columns)
@@ -238,16 +367,43 @@ extern "C" int esr_dcn_v2_backward(const float *input, const float *weight, cons
         if ((rc = conv_tc_launch(args, st))) return rc;
     }
     // 2. sampling backward
-    k_dcn_bwd_sample<<<(unsigned)ceil_div64((int64_t)px * 72, 256), 256, 0, st>>>(feat.base, feat.plane(), om, gcols, B, H, W, gin, gom);
-    ESR_LAUNCH_CHECK();
+    const unsigned wslices = (unsigned)ceil_div64((int64_t)px, WG_PSL);
+    if (!det) {
+        k_dcn_bwd_sample<<<(unsigned)ceil_div64((int64_t)px * 72, 256), 256, 0, st>>>(feat.base, feat.plane(), om, gcols, B, H, W, gin, gom);
+        ESR_LAUNCH_CHECK();
+    } else {
+        unsigned *maxw = (unsigned *)(ws + L.maxw);
+        unsigned long long *gin_q = (unsigned long long *)(ws + L.gin);
+        ESR_CUDA_CHECK(cudaMemsetAsync(maxw, 0, 4, st));
+        k_dcn_gin_max<<<(unsigned)min((int64_t)4096, ceil_div64((int64_t)px * 72, 256)), 256, 0, st>>>(om, gcols, px * 72, maxw);
+        ESR_LAUNCH_CHECK();
+        k_dcn_bwd_sample_det<<<(unsigned)ceil_div64((int64_t)px * 72, 256), 256, 0, st>>>(feat.base, feat.plane(), om, gcols, B, H, W,
+                                                                                          maxw, gin_q, gom);
+        ESR_LAUNCH_CHECK();
+    }
     // 3. weight / bias gradients (forward columns re-sampled)
     if ((rc = dcn_columns(feat, nullptr, om, B, cols, st))) return rc;
-    k_dcn_wgrad<<<dim3(9, (unsigned)ceil_div64((int64_t)px, WG_PSL)), 256, 0, st>>>(go_nhwc, cols.base, cols.plane(), px, grad_weight);
-    ESR_LAUNCH_CHECK();
-    k_dcn_bgrad<<<148, 256, 0, st>>>(go_nhwc, px, grad_bias);
-    ESR_LAUNCH_CHECK();
+    if (!det) {
+        k_dcn_wgrad<<<dim3(9, wslices), 256, 0, st>>>(go_nhwc, cols.base, cols.plane(), px, grad_weight);
+        ESR_LAUNCH_CHECK();
+        k_dcn_bgrad<<<BG_BLOCKS, 256, 0, st>>>(go_nhwc, px, grad_bias);
+        ESR_LAUNCH_CHECK();
+    } else {
+        float *wpart = (float *)(ws + L.wpart), *bpart = (float *)(ws + L.bpart);
+        k_dcn_wgrad_det<<<dim3(9, wslices), 256, 0, st>>>(go_nhwc, cols.base, cols.plane(), px, wpart);
+        ESR_LAUNCH_CHECK();
+        if ((rc = sum_slices(wpart, (int)wslices, 64 * 64 * 9, grad_weight, st))) return rc;
+        k_dcn_bgrad_det<<<BG_BLOCKS, 256, 0, st>>>(go_nhwc, px, bpart);
+        ESR_LAUNCH_CHECK();
+        if ((rc = sum_slices(bpart, BG_BLOCKS * 4, 64, grad_bias, st))) return rc;
+    }
     // back to the reference layouts
-    k_nhwc_to_nchw<<<(unsigned)ceil_div64((int64_t)px * 64, 256), 256, 0, st>>>(gin, B, 64, 0, 64, HW, grad_input);
+    if (!det) {
+        k_nhwc_to_nchw<<<(unsigned)ceil_div64((int64_t)px * 64, 256), 256, 0, st>>>(gin, B, 64, 0, 64, HW, grad_input);
+    } else {
+        k_dcn_gin_from_fixed<<<(unsigned)ceil_div64((int64_t)px * 64, 256), 256, 0, st>>>((const long long *)(ws + L.gin),
+                                                                                          (const unsigned *)(ws + L.maxw), B, HW, grad_input);
+    }
     ESR_LAUNCH_CHECK();
     k_nhwc_to_nchw<<<(unsigned)ceil_div64((int64_t)px * 144, 256), 256, 0, st>>>(gom, B, 144, 0, 216, HW, grad_offset);
     ESR_LAUNCH_CHECK();

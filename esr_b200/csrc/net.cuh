@@ -96,6 +96,10 @@ static inline bool dcn_is_tuned(int C, int Co, int kernel, int stride, int pad, 
     return C == 64 && Co == 64 && kernel == 3 && stride == 1 && pad == 1 && dil == 1 && G == 8;   // models/model.py:173
 }
 
+// out[i] = part[0][i] + part[1][i] + ... + part[slices-1][i] (part = [slices][n]), added in slot order: the second pass of
+// the deterministic reductions (train_ops.cu)
+int sum_slices(const float *part, int slices, size_t n, float *out, cudaStream_t st);
+
 // offset [B,144,HW] + mask [B,72,HW] (reference NCHW) -> om [B*HW, 216]
 int om_from_nchw(const float *offset, const float *mask, int B, int HW, float *om, cudaStream_t st);
 

@@ -14,8 +14,10 @@
 // bf16, 3-pass product, fp32 accumulate): the forward directly, dx as the same kernel over g with the weights transposed
 // and rotated, and dw as a tensor-core reduction over pixels (k_wgrad_tc below, MN-major operands).  Every other shape
 // (the <= 32-channel full-resolution layers, stride-2 encoder convs, 1- and 2-channel heads) uses the CUDA-core kernels
-// in this file.  dw / db / dx-by-atomics accumulate in fp32; summation order over pixels is not deterministic (neither is
-// the reference's cuDNN / atomicAdd backward).
+// in this file.  By default dw / db and the loss accumulate with fp32 atomics, so their summation order over pixels varies from
+// run to run (as the reference's cuDNN / atomicAdd backward does when cudnn.deterministic is off).  With ESR_DETERMINISTIC in
+// the flags of the _ex entry points every such sum goes through per-block partials and an ordered second pass instead, and
+// the results are bitwise reproducible on a given GPU model.
 #include "tc_common.cuh"
 #include "net.cuh"
 
@@ -45,8 +47,29 @@ __global__ void __launch_bounds__(256) k_act_bwd(const float *__restrict__ dy, c
     }
 }
 
-// db[co] += sum over (n, pixel) of g[n, co, pixel]; grid (Cout, chunks)
-__global__ void __launch_bounds__(256) k_bias_grad(const float *__restrict__ g, int B, int Cout, int HW, float *__restrict__ db)
+// Deterministic mode (ESR_DETERMINISTIC): every reduction over pixels that ends in fp32 atomics by default has a variant that
+// writes one partial per block (or per thread role) to slot s of a workspace buffer [slots][n] instead; k_sum_slices then adds
+// the slots in slot order.  The slot a partial lands in depends only on the launch geometry, never on CTA scheduling.
+// The variants share the kernel bodies below through a DET template parameter; the default kernels keep their names and code.
+__global__ void __launch_bounds__(256) k_sum_slices(const float *__restrict__ part, int slices, size_t n, float *__restrict__ out)
+{
+    for (size_t i = (size_t)blockIdx.x * 256 + threadIdx.x; i < n; i += (size_t)gridDim.x * 256) {
+        float s = 0.0f;
+        for (int k = 0; k < slices; ++k) s += part[(size_t)k * n + i];
+        out[i] = s;
+    }
+}
+
+int sum_slices(const float *part, int slices, size_t n, float *out, cudaStream_t st)
+{
+    k_sum_slices<<<(unsigned)min((size_t)2048, (n + 255) / 256), 256, 0, st>>>(part, slices, n, out);
+    ESR_LAUNCH_CHECK();
+    return ESR_OK;
+}
+
+// db[co] += sum over (n, pixel) of g[n, co, pixel]; grid (Cout, chunks).  DET: partial of block (co, chunk) -> db[chunk][co]
+template <bool DET>
+__device__ __forceinline__ void bias_grad_body(const float *__restrict__ g, int B, int Cout, int HW, float *__restrict__ db)
 {
     const int co = blockIdx.x;
     const size_t total = (size_t)B * HW;
@@ -62,8 +85,19 @@ __global__ void __launch_bounds__(256) k_bias_grad(const float *__restrict__ g, 
     if (threadIdx.x < 8) {
         s = red[threadIdx.x];
         for (int o = 4; o > 0; o >>= 1) s += __shfl_xor_sync(0xffu, s, o);
-        if (threadIdx.x == 0) atomicAdd(db + co, s);
+        if (threadIdx.x == 0) {
+            if (DET) db[(size_t)blockIdx.y * Cout + co] = s;
+            else atomicAdd(db + co, s);
+        }
     }
+}
+__global__ void __launch_bounds__(256) k_bias_grad(const float *__restrict__ g, int B, int Cout, int HW, float *__restrict__ db)
+{
+    bias_grad_body<false>(g, B, Cout, HW, db);
+}
+__global__ void __launch_bounds__(256) k_bias_grad_det(const float *__restrict__ g, int B, int Cout, int HW, float *__restrict__ part)
+{
+    bias_grad_body<true>(g, B, Cout, HW, part);
 }
 
 // wT[ci][co][K-1-ky][K-1-kx] = w[co][ci][ky][kx]: the weights of the convolution that maps g to dx (co padded to CoutPad)
@@ -354,11 +388,14 @@ __global__ void __launch_bounds__(256) k_conv_dgrad_s2(const float *__restrict__
 
 // dw for 3x3: thread = (input channel, kernel row) x 3 kernel columns x 8 output channels (24 accumulators), pixels of the
 // 16x16 tile split over 10 thread groups; 5 shared-memory instructions per 24 FMAs.
-__global__ void __launch_bounds__(256) k_conv_wgrad_r(const float *__restrict__ x, const float *__restrict__ g, float *__restrict__ dw,
-                                                      int B, int Cin, int H, int W, int Cout, int Ho, int Wo, int stride)
+// DET: the partial of pixel group `split` in block (pair, y) goes to slot y * WR_NSPLIT + split of dw = [slots][Cout*Cin*9].
+constexpr int WR_NSPLIT = 10;
+template <bool DET>
+__device__ __forceinline__ void wgrad_r_body(const float *__restrict__ x, const float *__restrict__ g, float *__restrict__ dw,
+                                             int B, int Cin, int H, int W, int Cout, int Ho, int Wo, int stride)
 {
     extern __shared__ float sm[];
-    constexpr int NR = G_C * 3, NSPLIT = 10;                       // 24 roles x 10 pixel groups = 240 threads
+    constexpr int NR = G_C * 3, NSPLIT = WR_NSPLIT;                // 24 roles x 10 pixel groups = 240 threads
     const int PD = (G_T - 1) * stride + 3;
     float *gs = sm;                                                // [256 px][G_C co]
     float *xs = sm + 256 * G_C;                                    // [G_C ci][PD][PD]
@@ -414,8 +451,21 @@ __global__ void __launch_bounds__(256) k_conv_wgrad_r(const float *__restrict__ 
         for (int k = 0; k < 3; ++k)
 #pragma unroll
             for (int c = 0; c < G_C; ++c)
-                if (co0 + c < Cout) atomicAdd(dw + ((size_t)(co0 + c) * Cin + ci0 + pci) * 9 + ky * 3 + k, acc[k][c]);
+                if (co0 + c < Cout) {
+                    if (DET) dw[((size_t)blockIdx.y * NSPLIT + split) * ((size_t)Cout * Cin * 9) + ((size_t)(co0 + c) * Cin + ci0 + pci) * 9 + ky * 3 + k] = acc[k][c];
+                    else atomicAdd(dw + ((size_t)(co0 + c) * Cin + ci0 + pci) * 9 + ky * 3 + k, acc[k][c]);
+                }
     }
+}
+__global__ void __launch_bounds__(256) k_conv_wgrad_r(const float *__restrict__ x, const float *__restrict__ g, float *__restrict__ dw,
+                                                      int B, int Cin, int H, int W, int Cout, int Ho, int Wo, int stride)
+{
+    wgrad_r_body<false>(x, g, dw, B, Cin, H, W, Cout, Ho, Wo, stride);
+}
+__global__ void __launch_bounds__(256) k_conv_wgrad_r_det(const float *__restrict__ x, const float *__restrict__ g, float *__restrict__ part,
+                                                          int B, int Cin, int H, int W, int Cout, int Ho, int Wo, int stride)
+{
+    wgrad_r_body<true>(x, g, part, B, Cin, H, W, Cout, Ho, Wo, stride);
 }
 
 __device__ __forceinline__ int floor_div(int a, int b) { return a >= 0 ? a / b : -((-a + b - 1) / b); }
@@ -475,9 +525,10 @@ __global__ void __launch_bounds__(256) k_conv_dgrad_g(const float *__restrict__ 
 
 // dw[co, ci, ky, kx] += sum over (n, oy, ox) of g[n, co, oy, ox] * x[n, ci, oy*s + ky - pad, ox*s + kx - pad]
 // grid (co-tiles * ci-tiles, work slices); each block walks (image, 16x16 output tile) items with stride gridDim.y
-template <int KS>
-__global__ void __launch_bounds__(256) k_conv_wgrad_g(const float *__restrict__ x, const float *__restrict__ g, float *__restrict__ dw,
-                                                      int B, int Cin, int H, int W, int Cout, int Ho, int Wo, int stride)
+// DET: the partial of pixel split `split` in block (pair, y) goes to slot y * (256 / (8 KS^2)) + split of dw = [slots][Cout*Cin*KK]
+template <int KS, bool DET>
+__device__ __forceinline__ void wgrad_g_body(const float *__restrict__ x, const float *__restrict__ g, float *__restrict__ dw,
+                                             int B, int Cin, int H, int W, int Cout, int Ho, int Wo, int stride)
 {
     extern __shared__ float sm[];
     constexpr int KK = KS * KS, pad = KS / 2, NP = G_C * KK;       // (ci, tap) pairs per block
@@ -527,8 +578,23 @@ __global__ void __launch_bounds__(256) k_conv_wgrad_g(const float *__restrict__ 
     if (active && ci0 + pci < Cin) {
 #pragma unroll
         for (int c = 0; c < G_C; ++c)
-            if (co0 + c < Cout) atomicAdd(dw + ((size_t)(co0 + c) * Cin + ci0 + pci) * KK + pt, acc[c]);
+            if (co0 + c < Cout) {
+                if (DET) dw[((size_t)blockIdx.y * NSPLIT + split) * ((size_t)Cout * Cin * KK) + ((size_t)(co0 + c) * Cin + ci0 + pci) * KK + pt] = acc[c];
+                else atomicAdd(dw + ((size_t)(co0 + c) * Cin + ci0 + pci) * KK + pt, acc[c]);
+            }
     }
+}
+template <int KS>
+__global__ void __launch_bounds__(256) k_conv_wgrad_g(const float *__restrict__ x, const float *__restrict__ g, float *__restrict__ dw,
+                                                      int B, int Cin, int H, int W, int Cout, int Ho, int Wo, int stride)
+{
+    wgrad_g_body<KS, false>(x, g, dw, B, Cin, H, W, Cout, Ho, Wo, stride);
+}
+template <int KS>
+__global__ void __launch_bounds__(256) k_conv_wgrad_g_det(const float *__restrict__ x, const float *__restrict__ g, float *__restrict__ part,
+                                                          int B, int Cin, int H, int W, int Cout, int Ho, int Wo, int stride)
+{
+    wgrad_g_body<KS, true>(x, g, part, B, Cin, H, W, Cout, Ho, Wo, stride);
 }
 
 // ------------------------------------------------------------------------------------------------------------------
@@ -751,8 +817,10 @@ __global__ void __launch_bounds__(256) k_gru_blend_bwd(const float *__restrict__
 // ------------------------------------------------------------------------------------------------------------------
 // loss and optimizer
 // ------------------------------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(256) k_mse(const float *__restrict__ p, const float *__restrict__ t, size_t n, float inv_n,
-                                             float *__restrict__ loss, float *__restrict__ grad, float grad_scale)
+// DET: block b writes its sum of squares to loss[b] (a workspace of gridDim.x floats); k_mse_finish adds them in block order
+template <bool DET>
+__device__ __forceinline__ void mse_body(const float *__restrict__ p, const float *__restrict__ t, size_t n, float inv_n,
+                                         float *__restrict__ loss, float *__restrict__ grad, float grad_scale)
 {
     float s = 0.0f;
     for (size_t i = (size_t)blockIdx.x * 256 + threadIdx.x; i < n; i += (size_t)gridDim.x * 256) {
@@ -767,8 +835,29 @@ __global__ void __launch_bounds__(256) k_mse(const float *__restrict__ p, const 
     if (threadIdx.x < 8) {
         s = red[threadIdx.x];
         for (int o = 4; o > 0; o >>= 1) s += __shfl_xor_sync(0xffu, s, o);
-        if (threadIdx.x == 0) atomicAdd(loss, s * inv_n);
+        if (threadIdx.x == 0) {
+            if (DET) loss[blockIdx.x] = s;
+            else atomicAdd(loss, s * inv_n);
+        }
     }
+}
+__global__ void __launch_bounds__(256) k_mse(const float *__restrict__ p, const float *__restrict__ t, size_t n, float inv_n,
+                                             float *__restrict__ loss, float *__restrict__ grad, float grad_scale)
+{
+    mse_body<false>(p, t, n, inv_n, loss, grad, grad_scale);
+}
+__global__ void __launch_bounds__(256) k_mse_det(const float *__restrict__ p, const float *__restrict__ t, size_t n, float inv_n,
+                                                 float *__restrict__ part, float *__restrict__ grad, float grad_scale)
+{
+    mse_body<true>(p, t, n, inv_n, part, grad, grad_scale);
+}
+// one warp: lane l adds partials l, l + 32, ... in order, then a fixed butterfly
+__global__ void k_mse_finish(const float *__restrict__ part, int blocks, float inv_n, float *__restrict__ loss)
+{
+    float s = 0.0f;
+    for (int i = threadIdx.x; i < blocks; i += 32) s += part[i];
+    for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+    if (threadIdx.x == 0) *loss = s * inv_n;
 }
 
 __global__ void k_adam_tick(int *step) { *step += 1; }
@@ -850,12 +939,47 @@ static int conv_tc_nchw(const float *x, const float *w, const float *bias, int B
     return conv_tc_launch(a, st);
 }
 
+// work slices (gridDim.y) of the CUDA-core weight-gradient kernels: about 8 blocks per SM, at most one per (image, tile) item
+static int wgrad_slices(int B, int Cin, int Cout, int Ho, int Wo)
+{
+    const int pairs = ((Cout + G_C - 1) / G_C) * ((Cin + G_C - 1) / G_C);
+    const int items = B * ((Wo + G_T - 1) / G_T) * ((Ho + G_T - 1) / G_T);
+    int slices = (dev_info().sm_count * 8 + pairs - 1) / pairs;
+    if (slices > items) slices = items;
+    if (slices < 1) slices = 1;
+    return slices;
+}
+// partial slots of the deterministic variant: per block, one per pixel split of k_conv_wgrad_r (3x3) / k_conv_wgrad_g<1> (1x1)
+static inline int wgrad_nsplit(int ksz) { return ksz == 3 ? WR_NSPLIT : 256 / G_C; }
+
+// which: 0 forward, 1 dx, 2 dw.  part (dw only): deterministic mode -- partials go to part, then an ordered sum into out.
 template <int KS>
 static int launch_generic(int which, const float *x, const float *w, const float *bias, const float *g, float *out, int B, int Cin,
-                          int H, int W, int Cout, int Ho, int Wo, int stride, int act, cudaStream_t st)
+                          int H, int W, int Cout, int Ho, int Wo, int stride, int act, cudaStream_t st, float *part = nullptr)
 {
     constexpr int KK = KS * KS;
     const dim3 blk(G_T, G_T);
+    if (which == 2 && part) {
+        if (KS == 3 && getenv("ESR_WGRAD_MMA") != nullptr) {
+            set_error("conv2d_backward: the ESR_WGRAD_MMA weight gradient sums with atomics and has no deterministic variant; "
+                      "unset ESR_WGRAD_MMA or leave deterministic mode");
+            return ESR_EUNSUPPORTED;
+        }
+        const int PD = (G_T - 1) * stride + KS;
+        const size_t smem = (size_t)(256 * G_C + G_C * PD * PD) * 4;
+        const int pairs = ((Cout + G_C - 1) / G_C) * ((Cin + G_C - 1) / G_C);
+        const int slices = wgrad_slices(B, Cin, Cout, Ho, Wo);
+        static bool attr = false;
+        if constexpr (KS == 3) {
+            if (!attr) { ESR_CUDA_CHECK(cudaFuncSetAttribute(k_conv_wgrad_r_det, cudaFuncAttributeMaxDynamicSharedMemorySize, 64 * 1024)); attr = true; }
+            k_conv_wgrad_r_det<<<dim3(pairs, slices), 256, smem, st>>>(x, g, part, B, Cin, H, W, Cout, Ho, Wo, stride);
+        } else {
+            if (!attr) { ESR_CUDA_CHECK(cudaFuncSetAttribute(k_conv_wgrad_g_det<KS>, cudaFuncAttributeMaxDynamicSharedMemorySize, 64 * 1024)); attr = true; }
+            k_conv_wgrad_g_det<KS><<<dim3(pairs, slices), 256, smem, st>>>(x, g, part, B, Cin, H, W, Cout, Ho, Wo, stride);
+        }
+        ESR_LAUNCH_CHECK();
+        return sum_slices(part, slices * wgrad_nsplit(KS), (size_t)Cout * Cin * KK, out, st);
+    }
     if (which == 0 && KS == 3 && stride == 1) {
         const size_t smem = (size_t)(G_C * R_PH * R_PW + G_C * 9 * G_C) * 4;
         const dim3 grid(((Wo + R_TW - 1) / R_TW) * ((Ho + R_TH - 1) / R_TH), (Cout + G_C - 1) / G_C, B);
@@ -921,14 +1045,49 @@ static int launch_generic(int which, const float *x, const float *w, const float
 }
 
 static int generic(int which, int ksz, const float *x, const float *w, const float *bias, const float *g, float *out, int B, int Cin,
-                   int H, int W, int Cout, int Ho, int Wo, int stride, int act, cudaStream_t st)
+                   int H, int W, int Cout, int Ho, int Wo, int stride, int act, cudaStream_t st, float *part = nullptr)
 {
-    return ksz == 3 ? launch_generic<3>(which, x, w, bias, g, out, B, Cin, H, W, Cout, Ho, Wo, stride, act, st)
-                    : launch_generic<1>(which, x, w, bias, g, out, B, Cin, H, W, Cout, Ho, Wo, stride, act, st);
+    return ksz == 3 ? launch_generic<3>(which, x, w, bias, g, out, B, Cin, H, W, Cout, Ho, Wo, stride, act, st, part)
+                    : launch_generic<1>(which, x, w, bias, g, out, B, Cin, H, W, Cout, Ho, Wo, stride, act, st, part);
 }
 
+// db = sum of g over (image, pixel); part != NULL: deterministic (per-block partials, then the ordered sum)
+static int bias_grad(const float *g, int B, int Cout, int HW, float *db, float *part, cudaStream_t st)
+{
+    const size_t total = (size_t)B * HW;
+    int chunks = (int)min((size_t)64, (total + 4095) / 4096);
+    if (chunks < 1) chunks = 1;
+    if (!part) {
+        k_bias_grad<<<dim3(Cout, chunks), 256, 0, st>>>(g, B, Cout, HW, db);
+        ESR_LAUNCH_CHECK();
+        return ESR_OK;
+    }
+    k_bias_grad_det<<<dim3(Cout, chunks), 256, 0, st>>>(g, B, Cout, HW, part);
+    ESR_LAUNCH_CHECK();
+    return sum_slices(part, chunks, (size_t)Cout, db, st);
+}
+
+// wgrad_tc.cu (returns ESR_EINVAL when the shape is not supported).  part != NULL: deterministic (see wgrad_tc_part_bytes)
 int wgrad_tc(const __nv_bfloat16 *x_split, const __nv_bfloat16 *g_split, int B, int Cin, int H, int W, int Cout, int CoutPad, int ksz,
-             float *dw, cudaStream_t st);   // wgrad_tc.cu (returns ESR_EINVAL when the shape is not supported)
+             float *dw, float *part, cudaStream_t st);
+size_t wgrad_tc_part_bytes(int B, int Cin, int H, int W, int Cout, int CoutPad, int ksz);
+
+// the dw kernel esr_conv2d_backward picks: k_wgrad_tc for the 64-multiple layers, the CUDA-core kernels otherwise
+static inline bool use_tc_dw(int Cin, int Cout, int ksz, int stride)
+{
+    return tc_dgrad_ok(Cin, Cout, ksz, stride) && Cin % 64 == 0 && getenv("ESR_WGRAD_GENERIC") == nullptr;
+}
+
+// deterministic mode's extra workspace, after the default layout: bias partials (<= 64 chunks), then the dw partials
+static size_t conv2d_det_bias_bytes(int Cout) { return align_up((size_t)64 * Cout * 4, 256); }
+static size_t conv2d_det_bytes(int B, int Cin, int H, int W, int Cout, int ksz, int stride)
+{
+    const int Ho = (H + 2 * (ksz / 2) - ksz) / stride + 1, Wo = (W + 2 * (ksz / 2) - ksz) / stride + 1;
+    const size_t dw = use_tc_dw(Cin, Cout, ksz, stride)
+                          ? wgrad_tc_part_bytes(B, Cin, H, W, Cout, pad64(Cout), ksz)
+                          : (size_t)wgrad_slices(B, Cin, Cout, Ho, Wo) * wgrad_nsplit(ksz) * Cout * Cin * ksz * ksz * 4;
+    return conv2d_det_bias_bytes(Cout) + dw;
+}
 
 } // namespace esr
 
@@ -939,6 +1098,12 @@ extern "C" {
 size_t esr_conv2d_workspace_bytes(int B, int Cin, int H, int W, int Cout, int ksz, int stride)
 {
     return conv2d_ws(B, Cin, H, W, Cout, ksz, stride);
+}
+
+size_t esr_conv2d_workspace_bytes_ex(int B, int Cin, int H, int W, int Cout, int ksz, int stride, int flags)
+{
+    const size_t base = conv2d_ws(B, Cin, H, W, Cout, ksz, stride);
+    return (flags & ESR_DETERMINISTIC) ? base + conv2d_det_bytes(B, Cin, H, W, Cout, ksz, stride) : base;
 }
 
 size_t esr_conv2d_split_bytes(int B, int Cin, int H, int W, int Cout, int ksz, int stride)
@@ -976,6 +1141,14 @@ int esr_conv2d_backward(const float *x, const void *x_split, const float *w, con
                         int W, int Cout, int ksz, int stride, int act, float *dx, float *dw, float *db, void *workspace,
                         size_t workspace_bytes, esr_stream_t stream)
 {
+    return esr_conv2d_backward_ex(x, x_split, w, y, dy, B, Cin, H, W, Cout, ksz, stride, act, dx, dw, db, 0, workspace, workspace_bytes,
+                                  stream);
+}
+
+int esr_conv2d_backward_ex(const float *x, const void *x_split, const float *w, const float *y, const float *dy, int B, int Cin, int H,
+                           int W, int Cout, int ksz, int stride, int act, float *dx, float *dw, float *db, int flags, void *workspace,
+                           size_t workspace_bytes, esr_stream_t stream)
+{
     cudaStream_t st = (cudaStream_t)stream;
     ESR_REQUIRE((x || x_split) && w && dy && workspace && ((dw && db) || (!dw && !db && dx)), "conv2d_backward: null pointer");
     ESR_REQUIRE(!x_split || esr_conv2d_split_bytes(B, Cin, H, W, Cout, ksz, stride) > 0, "conv2d_backward: x_split given for a layer without a tensor-core dw");
@@ -985,12 +1158,22 @@ int esr_conv2d_backward(const float *x, const void *x_split, const float *w, con
     ESR_REQUIRE((ksz == 3 || ksz == 1) && (stride == 1 || stride == 2) && act >= 0 && act <= 3, "conv2d_backward: ksz=%d stride=%d act=%d", ksz,
                 stride, act);
     const int pad = ksz / 2, Ho = (H + 2 * pad - ksz) / stride + 1, Wo = (W + 2 * pad - ksz) / stride + 1;
-    Bump ws{(uint8_t *)workspace, 0, workspace_bytes};
+    // deterministic mode: the partial buffers sit after the default layout (esr_conv2d_workspace_bytes_ex)
+    const bool det = (flags & ESR_DETERMINISTIC) != 0;
+    const size_t base_bytes = conv2d_ws(B, Cin, H, W, Cout, ksz, stride);
+    float *bias_part = nullptr, *dw_part = nullptr;
+    if (det && want_dw) {
+        ESR_REQUIRE(workspace_bytes >= base_bytes + conv2d_det_bytes(B, Cin, H, W, Cout, ksz, stride),
+                    "conv2d_backward: deterministic mode needs esr_conv2d_workspace_bytes_ex(..., ESR_DETERMINISTIC) bytes");
+        bias_part = (float *)((uint8_t *)workspace + base_bytes);
+        dw_part = (float *)((uint8_t *)workspace + base_bytes + conv2d_det_bias_bytes(Cout));
+    }
+    Bump ws{(uint8_t *)workspace, 0, det ? base_bytes : workspace_bytes};
     int rc;
     const size_t ng = (size_t)B * Cout * Ho * Wo;
     const bool tcd = tc_dgrad_ok(Cin, Cout, ksz, stride);
     const int gC = pad64(Cout);
-    const bool tc_dw = tcd && Cin % 64 == 0 && getenv("ESR_WGRAD_GENERIC") == nullptr;
+    const bool tc_dw = tcd && use_tc_dw(Cin, Cout, ksz, stride);
     float *g = (float *)ws.take(ng * 4);                           // fp32 g: only the CUDA-core kernels read it
     __nv_bfloat16 *gsplit = nullptr;
     if (want_dw) {
@@ -998,14 +1181,16 @@ int esr_conv2d_backward(const float *x, const void *x_split, const float *w, con
         ESR_CUDA_CHECK(cudaMemsetAsync(dw, 0, (size_t)Cout * Cin * ksz * ksz * 4, st));
     }
     if (tcd) {
-        // one pass: activation derivative, bias gradient, fp32 -> split bf16 NHWC (padded to a 64-multiple of channels)
+        // one pass: activation derivative, bias gradient, fp32 -> split bf16 NHWC (padded to a 64-multiple of channels).
+        // Deterministic mode: the pass writes fp32 g instead of adding db, and db is summed from g in a fixed order below.
         gsplit = (__nv_bfloat16 *)ws.take((size_t)B * gC * Ho * Wo * 4);
         ESR_REQUIRE(ws.off <= ws.cap, "conv2d_backward: workspace too small");
         const int tpb = split_tiles_per_block(Ho * Wo, gC / 64, B), tiles = (Ho * Wo + 31) / 32;
         k_to_split<true><<<dim3((tiles + tpb - 1) / tpb, gC / 64, B), 256, 0, st>>>(dy, y, act, Cout, gC, Ho * Wo, tpb, gsplit,
-                                                                                   (size_t)B * Ho * Wo * gC, want_dw ? db : nullptr,
-                                                                                   tc_dw ? nullptr : g);
+                                                                                   (size_t)B * Ho * Wo * gC, want_dw && !det ? db : nullptr,
+                                                                                   tc_dw && !(det && want_dw) ? nullptr : g);
         ESR_LAUNCH_CHECK();
+        if (det && want_dw && (rc = bias_grad(g, B, Cout, Ho * Wo, db, bias_part, st))) return rc;
     } else {
         ESR_REQUIRE(ws.off <= ws.cap, "conv2d_backward: workspace too small");
         if (act == ACT_NONE) {
@@ -1014,12 +1199,7 @@ int esr_conv2d_backward(const float *x, const void *x_split, const float *w, con
             k_act_bwd<<<(unsigned)min((size_t)4096, (ng + 255) / 256), 256, 0, st>>>(dy, y, g, ng, act);
             ESR_LAUNCH_CHECK();
         }
-        if (want_dw) {
-            const size_t total = (size_t)B * Ho * Wo;
-            int chunks = (int)min((size_t)64, (total + 4095) / 4096);
-            k_bias_grad<<<dim3(Cout, chunks < 1 ? 1 : chunks), 256, 0, st>>>(g, B, Cout, Ho * Wo, db);
-            ESR_LAUNCH_CHECK();
-        }
+        if (want_dw && (rc = bias_grad(g, B, Cout, Ho * Wo, db, bias_part, st))) return rc;
     }
     // ---- dw
     bool dw_done = !want_dw;
@@ -1032,10 +1212,10 @@ int esr_conv2d_backward(const float *x, const void *x_split, const float *w, con
             if ((rc = split_from_nchw_pad(x, B, Cin, Cin, H * W, xs_, st))) return rc;
             xsplit = xs_;
         }
-        if ((rc = wgrad_tc(xsplit, gsplit, B, Cin, H, W, Cout, gC, ksz, dw, st))) return rc;   // (fp32 g was not written)
+        if ((rc = wgrad_tc(xsplit, gsplit, B, Cin, H, W, Cout, gC, ksz, dw, dw_part, st))) return rc;
         dw_done = true;
     }
-    if (!dw_done && (rc = generic(2, ksz, x, nullptr, nullptr, g, dw, B, Cin, H, W, Cout, Ho, Wo, stride, 0, st))) return rc;
+    if (!dw_done && (rc = generic(2, ksz, x, nullptr, nullptr, g, dw, B, Cin, H, W, Cout, Ho, Wo, stride, 0, st, dw_part))) return rc;
     // ---- dx
     if (dx) {
         if (tcd) {
@@ -1139,6 +1319,28 @@ int esr_mse_loss(const float *pred, const float *target, size_t n, float *loss, 
     ESR_REQUIRE(pred && target && loss && n > 0, "mse_loss: bad arguments");
     ESR_CUDA_CHECK(cudaMemsetAsync(loss, 0, 4, st));
     k_mse<<<(unsigned)min((size_t)1024, (n + 255) / 256), 256, 0, st>>>(pred, target, n, 1.0f / (float)n, loss, grad, grad_scale);
+    ESR_LAUNCH_CHECK();
+    return ESR_OK;
+}
+
+size_t esr_mse_loss_workspace_bytes_ex(size_t n, int flags)
+{
+    (void)n;
+    return (flags & ESR_DETERMINISTIC) ? 1024 * sizeof(float) : 0;  // one partial per block (at most 1024 blocks)
+}
+
+int esr_mse_loss_ex(const float *pred, const float *target, size_t n, float *loss, float *grad, float grad_scale, int flags,
+                    void *workspace, size_t workspace_bytes, esr_stream_t stream)
+{
+    if (!(flags & ESR_DETERMINISTIC)) return esr_mse_loss(pred, target, n, loss, grad, grad_scale, stream);
+    cudaStream_t st = (cudaStream_t)stream;
+    ESR_REQUIRE(pred && target && loss && n > 0, "mse_loss: bad arguments");
+    ESR_REQUIRE(workspace && workspace_bytes >= esr_mse_loss_workspace_bytes_ex(n, flags), "mse_loss: workspace too small");
+    const unsigned blocks = (unsigned)min((size_t)1024, (n + 255) / 256);
+    float *part = (float *)workspace;
+    k_mse_det<<<blocks, 256, 0, st>>>(pred, target, n, 1.0f / (float)n, part, grad, grad_scale);
+    ESR_LAUNCH_CHECK();
+    k_mse_finish<<<1, 32, 0, st>>>(part, (int)blocks, 1.0f / (float)n, loss);
     ESR_LAUNCH_CHECK();
     return ESR_OK;
 }

@@ -34,7 +34,10 @@ struct WgradArgs {
     int n_img, H, W, TW, TH, tiles_x, tiles_y, slices;
 };
 
-__global__ void __launch_bounds__(WG_THREADS, 1) k_wgrad_tc(const __grid_constant__ WgradArgs a)
+// DET: instead of the atomics, the CTA of slice s stores its tile to slot s of a.dw = [slices][Cout*Cin*KK] (every CTA of a
+// slice owns distinct elements, and every slice walks at least one tile, so each slot is written in full); sum_slices adds them.
+template <bool DET>
+__device__ __forceinline__ void wgrad_tc_body(const WgradArgs &a)
 {
     extern __shared__ uint8_t smem_raw[];
     const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
@@ -166,14 +169,53 @@ __global__ void __launch_bounds__(WG_THREADS, 1) k_wgrad_tc(const __grid_constan
             const int nc = n0 + 8 * (i >> 2) + 2 * (lane & 3) + (i & 1);        // column = N-side channel
             const bool row_ok = (m < 64 || !m_dup) && (m0 + m < m_real);
             const int co = a.a_is_x ? nc : m0 + m, ci = a.a_is_x ? m0 + m : nc;
-            if (row_ok && co < a.Cout) atomicAdd(a.dw + ((size_t)co * a.Cin + ci) * a.KK + tap, acc[j][i]);
+            if (row_ok && co < a.Cout) {
+                if (DET) a.dw[(size_t)slice * a.Cout * a.Cin * a.KK + ((size_t)co * a.Cin + ci) * a.KK + tap] = acc[j][i];
+                else atomicAdd(a.dw + ((size_t)co * a.Cin + ci) * a.KK + tap, acc[j][i]);
+            }
         }
     }
 }
+__global__ void __launch_bounds__(WG_THREADS, 1) k_wgrad_tc(const __grid_constant__ WgradArgs a) { wgrad_tc_body<false>(a); }
+__global__ void __launch_bounds__(WG_THREADS, 1) k_wgrad_tc_det(const __grid_constant__ WgradArgs a) { wgrad_tc_body<true>(a); }
+
+// CTAs per (M block, N chunk, tap group): one CTA per SM in all.  (Every CTA ends with 128 x 64 x taps fp32 atomics; giving small
+// problems fewer, longer CTAs was measured slower: min 6 tiles per CTA +0.3 ms, min 16 +2 ms per cfg2 training iteration --
+// ESR_WGRAD_MIN_TILES to retest.)
+static int wgrad_tc_slices(int n_tiles, int base)
+{
+    int slices = (dev_info().sm_count + base - 1) / base;
+    static const int min_tiles = getenv("ESR_WGRAD_MIN_TILES") ? atoi(getenv("ESR_WGRAD_MIN_TILES")) : 1;
+    if (slices > n_tiles / min_tiles) slices = n_tiles / min_tiles;
+    if (slices < 1) slices = 1;
+    return slices;
+}
+
+static void wgrad_tc_geometry(int B, int Cin, int H, int W, int Cout, int CoutPad, int ksz, WgradArgs &a)
+{
+    a.Cout = Cout; a.Cin = Cin; a.KK = ksz * ksz; a.CoutPad = CoutPad;
+    a.a_is_x = (Cout == 64 && Cin >= 128) ? 1 : 0;
+    a.TW = W >= 24 ? 32 : (W >= 12 ? 16 : 8); a.TH = TC_BLOCK_M / a.TW;
+    const int m_ch = a.a_is_x ? Cin : CoutPad, n_ch = a.a_is_x ? CoutPad : Cin;
+    a.m_blocks = (m_ch + 127) / 128; a.n_chunks = n_ch / 64; a.groups = ksz == 3 ? 9 / WG_TAPS : 1;
+    a.n_img = B; a.H = H; a.W = W;
+    a.tiles_x = (W + a.TW - 1) / a.TW; a.tiles_y = (H + a.TH - 1) / a.TH;
+    a.slices = wgrad_tc_slices(B * a.tiles_x * a.tiles_y, a.m_blocks * a.n_chunks * a.groups);
+}
+
+// partial buffer of the deterministic variant: [slices][Cout][Cin][KK] fp32
+size_t wgrad_tc_part_bytes(int B, int Cin, int H, int W, int Cout, int CoutPad, int ksz)
+{
+    WgradArgs a;
+    memset(&a, 0, sizeof(a));
+    wgrad_tc_geometry(B, Cin, H, W, Cout, CoutPad, ksz, a);
+    return (size_t)a.slices * Cout * Cin * ksz * ksz * 4;
+}
 
 // x_split: split NHWC [2][B][H][W][Cin]; g_split: split NHWC [2][B][H][W][CoutPad] (channels >= Cout zero); dw pre-zeroed.
+// part != NULL: deterministic mode -- per-slice partial tiles into part (wgrad_tc_part_bytes), then the ordered sum into dw.
 int wgrad_tc(const __nv_bfloat16 *x_split, const __nv_bfloat16 *g_split, int B, int Cin, int H, int W, int Cout, int CoutPad, int ksz,
-             float *dw, cudaStream_t st)
+             float *dw, float *part, cudaStream_t st)
 {
     if (Cin % 64 != 0 || CoutPad % 64 != 0 || CoutPad < Cout || (ksz != 3 && ksz != 1)) return ESR_EINVAL;
     int rc;
@@ -181,33 +223,29 @@ int wgrad_tc(const __nv_bfloat16 *x_split, const __nv_bfloat16 *g_split, int B, 
     SplitTensor gs; gs.base = const_cast<__nv_bfloat16 *>(g_split); gs.n_img = B; gs.H = H; gs.W = W; gs.C = CoutPad;
     WgradArgs a;
     memset(&a, 0, sizeof(a));
-    a.dw = dw; a.Cout = Cout; a.Cin = Cin; a.KK = ksz * ksz;
-    a.a_is_x = (Cout == 64 && Cin >= 128) ? 1 : 0;
-    a.TW = W >= 24 ? 32 : (W >= 12 ? 16 : 8); a.TH = TC_BLOCK_M / a.TW;
+    wgrad_tc_geometry(B, Cin, H, W, Cout, CoutPad, ksz, a);
+    a.dw = part ? part : dw;
     if ((rc = tc_make_amap(gs, a.TW, a.TH, &a.gmap))) return rc;
     if ((rc = tc_make_amap(xs, a.TW, a.TH, &a.xmap))) return rc;
-    const int m_ch = a.a_is_x ? Cin : CoutPad, n_ch = a.a_is_x ? CoutPad : Cin;
-    a.CoutPad = CoutPad;
-    a.m_blocks = (m_ch + 127) / 128; a.n_chunks = n_ch / 64; a.groups = ksz == 3 ? 9 / WG_TAPS : 1;
-    a.n_img = B; a.H = H; a.W = W;
-    a.tiles_x = (W + a.TW - 1) / a.TW; a.tiles_y = (H + a.TH - 1) / a.TH;
-    const int n_tiles = B * a.tiles_x * a.tiles_y, base = a.m_blocks * a.n_chunks * a.groups;
-    // one CTA per SM.  (Every CTA ends with 128 x 64 x taps fp32 atomics; giving small problems fewer, longer CTAs was measured
-    // slower: min 6 tiles per CTA +0.3 ms, min 16 +2 ms per cfg2 training iteration -- ESR_WGRAD_MIN_TILES to retest.)
-    int slices = (dev_info().sm_count + base - 1) / base;
-    static const int min_tiles = getenv("ESR_WGRAD_MIN_TILES") ? atoi(getenv("ESR_WGRAD_MIN_TILES")) : 1;
-    if (slices > n_tiles / min_tiles) slices = n_tiles / min_tiles;
-    if (slices < 1) slices = 1;
-    a.slices = slices;
+    const int base = a.m_blocks * a.n_chunks * a.groups;
     const size_t smem = 1024 + 2 * (size_t)(4 * WG_TILE) + 2 * (size_t)(2 * WG_TILE) + 64;
-    static size_t attr_done = 0;
-    if (smem > attr_done) {
-        ESR_CUDA_CHECK(cudaFuncSetAttribute(k_wgrad_tc, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        attr_done = smem;
+    static size_t attr_done = 0, attr_det = 0;
+    if (!part) {
+        if (smem > attr_done) {
+            ESR_CUDA_CHECK(cudaFuncSetAttribute(k_wgrad_tc, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+            attr_done = smem;
+        }
+        k_wgrad_tc<<<(unsigned)(base * a.slices), WG_THREADS, smem, st>>>(a);
+        ESR_LAUNCH_CHECK();
+        return ESR_OK;
     }
-    k_wgrad_tc<<<(unsigned)(base * slices), WG_THREADS, smem, st>>>(a);
+    if (smem > attr_det) {
+        ESR_CUDA_CHECK(cudaFuncSetAttribute(k_wgrad_tc_det, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        attr_det = smem;
+    }
+    k_wgrad_tc_det<<<(unsigned)(base * a.slices), WG_THREADS, smem, st>>>(a);
     ESR_LAUNCH_CHECK();
-    return ESR_OK;
+    return sum_slices(part, a.slices, (size_t)Cout * Cin * ksz * ksz, dw, st);
 }
 
 } // namespace esr

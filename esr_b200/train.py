@@ -31,6 +31,18 @@ def _ws(nbytes, device):
     return torch.empty((max(int(nbytes), 256),), dtype=torch.uint8, device=device)
 
 
+def deterministic():
+    """True when the training operators must be bitwise reproducible: torch.use_deterministic_algorithms(True) or
+    torch.backends.cudnn.deterministic = True (the reference trainer's init_seeds sets the latter, train_ours_cnt_seq.py:30-46).
+    Read at every call.  In this mode every gradient / loss reduction runs from per-block partials in a fixed order (or in
+    int64 fixed point for the DCN grad_input), and paths that have no such variant raise ESRError."""
+    return torch.are_deterministic_algorithms_enabled() or bool(torch.backends.cudnn.deterministic)
+
+
+def _flags():
+    return _lib.DETERMINISTIC if deterministic() else 0
+
+
 _DEFERRED = None        # None: off.  dict key -> [sink, [(x, y, dy), ...]] while a train_step collects weight-shared layers
 
 
@@ -74,12 +86,13 @@ def _conv2d_backward_raw(x, w, y, dy, stride, act, need_dx=True, need_dw=True, x
     dx = torch.empty((B, Cin, H, W), dtype=torch.float32, device=w.device) if need_dx else None
     dw = torch.empty_like(w) if need_dw else None
     db = torch.empty((Cout,), dtype=torch.float32, device=w.device) if need_dw else None
+    flags = _flags()
     with torch.cuda.device(w.device):
-        nbytes = L.esr_conv2d_workspace_bytes(B, Cin, H, W, Cout, k, stride)
+        nbytes = L.esr_conv2d_workspace_bytes_ex(B, Cin, H, W, Cout, k, stride, flags)
         ws = _ws(nbytes, w.device)
-        _lib.check(L.esr_conv2d_backward(_lib.ptr(x), _lib.ptr(x_split), _lib.ptr(w), _lib.ptr(y), _lib.ptr(dy), B, Cin, H, W, Cout, k, stride,
-                                         act, _lib.ptr(dx), _lib.ptr(dw), _lib.ptr(db), _lib.ptr(ws), nbytes,
-                                         _lib.stream_ptr()), "esr_conv2d_backward")
+        _lib.check(L.esr_conv2d_backward_ex(_lib.ptr(x), _lib.ptr(x_split), _lib.ptr(w), _lib.ptr(y), _lib.ptr(dy), B, Cin, H, W, Cout, k,
+                                            stride, act, _lib.ptr(dx), _lib.ptr(dw), _lib.ptr(db), flags, _lib.ptr(ws), nbytes,
+                                            _lib.stream_ptr()), "esr_conv2d_backward")
     return dx, dw, db
 
 
@@ -231,9 +244,12 @@ class _MSEFn(torch.autograd.Function):
         pred, target = pred.contiguous().float(), target.contiguous().float()
         loss = torch.empty((1,), dtype=torch.float32, device=pred.device)
         grad = torch.empty_like(pred)
+        flags, L = _flags(), _lib.lib()
         with torch.cuda.device(pred.device):
-            _lib.check(_lib.lib().esr_mse_loss(_lib.ptr(pred), _lib.ptr(target), pred.numel(), _lib.ptr(loss), _lib.ptr(grad),
-                                               1.0, _lib.stream_ptr()), "esr_mse_loss")
+            nbytes = L.esr_mse_loss_workspace_bytes_ex(pred.numel(), flags)
+            ws = _ws(nbytes, pred.device) if nbytes else None
+            _lib.check(L.esr_mse_loss_ex(_lib.ptr(pred), _lib.ptr(target), pred.numel(), _lib.ptr(loss), _lib.ptr(grad), 1.0, flags,
+                                         _lib.ptr(ws), nbytes, _lib.stream_ptr()), "esr_mse_loss")
         ctx.save_for_backward(grad)
         return loss[0]
 
@@ -537,10 +553,13 @@ def train_step(model, optimizer, frames, gt, num_frame=None, all_reduce=None):
 
 class GraphedTrainStep:
     """train_step captured once into a CUDA graph (forward, backward, all-reduce hook and the Adam kernel) and replayed:
-    no Python / launch overhead per iteration.  Shapes are fixed at construction; data is copied into static buffers."""
+    no Python / launch overhead per iteration.  Shapes are fixed at construction; data is copied into static buffers.
+    The graph holds the kernels of the mode it was captured in (`deterministic()` or not); replaying it after the mode has
+    changed raises ESRError instead of running the other mode's kernels."""
 
     def __init__(self, model, optimizer, frames_shape, device, num_frame=None, all_reduce=None, warmup=2):
         self.model, self.opt = model, optimizer
+        self.deterministic = deterministic()
         num_frame = _model_num_frame(model, num_frame)
         self.frames = torch.zeros(frames_shape, dtype=torch.float32, device=device)
         self.gt = torch.zeros(frames_shape, dtype=torch.float32, device=device)
@@ -579,6 +598,10 @@ class GraphedTrainStep:
             raise err
 
     def __call__(self, frames, gt):
+        if deterministic() != self.deterministic:
+            raise _lib.ESRError(f"GraphedTrainStep was captured with deterministic mode {'on' if self.deterministic else 'off'}; "
+                                "restore torch.use_deterministic_algorithms / torch.backends.cudnn.deterministic to that "
+                                "setting or capture a new GraphedTrainStep")
         self.frames.copy_(frames)
         self.gt.copy_(gt)
         self.opt.upload_hyper()                                   # a scheduler may have changed param_groups[0]['lr']

@@ -25,6 +25,13 @@ extern "C" {
 #define ESR_EUNSUPPORTED (-4) /* configuration outside what the sm_90a kernels implement */
 #define ESR_EWORKSPACE (-5)   /* workspace too small */
 
+/* `flags` bits of the *_ex training entry points.  ESR_DETERMINISTIC: every reduction that sums with fp32 atomics by default
+ * (bias and weight gradients, the loss, the deformable convolution's grad_input) runs as per-block partials added in a fixed
+ * order, or in int64 fixed point, so repeated calls on the same GPU model give bitwise identical results -- what
+ * torch.backends.cudnn.deterministic / torch.use_deterministic_algorithms ask of cuDNN.  Paths without such a variant return
+ * ESR_EUNSUPPORTED in this mode.  The workspace queries with the same flags include the partial buffers. */
+#define ESR_DETERMINISTIC 1
+
 typedef void *esr_stream_t; /* cudaStream_t */
 
 int esr_version(void);
@@ -281,12 +288,25 @@ size_t esr_dcn_v2_workspace_bytes_ex(int B, int C, int H, int W, int Co, int ker
 /* Replaces: models/DCNv2/src/dcn_v2.h:29-50 dcn_v2_backward -> src/cuda/dcn_v2_cuda.cu:97-216 (+ the col2im / coord kernels
  * src/cuda/dcn_v2_im2col_cuda.cu:197-327), called from models/DCNv2/dcn_v2.py:50.  Same five gradients, reference layouts:
  * grad_input [B,C,H,W], grad_offset [B,dg*18,H,W], grad_mask [B,dg*9,H,W], grad_weight [Co,C,3,3], grad_bias [Co].
- * grad_input uses fp32 atomics like the reference (summation order is not deterministic). */
+ * By default grad_input, grad_weight and grad_bias sum with fp32 atomics like the reference, so their summation order varies
+ * from call to call; esr_dcn_v2_backward_ex with ESR_DETERMINISTIC makes them bitwise reproducible. */
 size_t esr_dcn_v2_backward_workspace_bytes(int B, int H, int W);
 int esr_dcn_v2_backward(const float *input, const float *weight, const float *bias, const float *offset, const float *mask,
                         const float *grad_output, int B, int C, int H, int W, int Co, int kernel, int stride, int pad,
                         int dilation, int deformable_group, float *grad_input, float *grad_offset, float *grad_mask,
                         float *grad_weight, float *grad_bias, void *workspace, size_t workspace_bytes, esr_stream_t stream);
+/* Replaces the same dcn_v2_backward (models/DCNv2/src/dcn_v2.h:29-50, called from models/DCNv2/dcn_v2.py:50) with `flags`
+ * (ESR_DETERMINISTIC or 0; 0 is esr_dcn_v2_backward).  Deterministic mode: grad_input accumulates in int64 fixed point (scale
+ * chosen from the largest |grad_columns * mask| of the call so that no element can overflow), grad_weight / grad_bias from
+ * per-slice partials.  Only the configuration of models/model.py:173 has this mode; any other returns ESR_EUNSUPPORTED.
+ * Workspace: esr_dcn_v2_backward_workspace_bytes_ex with the same configuration and flags. */
+size_t esr_dcn_v2_backward_workspace_bytes_ex(int B, int C, int H, int W, int Co, int kernel, int stride, int pad, int dilation,
+                                              int deformable_group, int flags);
+int esr_dcn_v2_backward_ex(const float *input, const float *weight, const float *bias, const float *offset, const float *mask,
+                           const float *grad_output, int B, int C, int H, int W, int Co, int kernel, int stride, int pad,
+                           int dilation, int deformable_group, float *grad_input, float *grad_offset, float *grad_mask,
+                           float *grad_weight, float *grad_bias, int flags, void *workspace, size_t workspace_bytes,
+                           esr_stream_t stream);
 int esr_dcn_v2_forward(const float *input, const float *weight, const float *bias, const float *offset, const float *mask,
                        int B, int C, int H, int W, int Co, int kernel, int stride, int pad, int dilation,
                        int deformable_group, float *output, void *workspace, size_t workspace_bytes, esr_stream_t stream);
@@ -313,6 +333,14 @@ int esr_conv2d_forward(const float *x, const float *w, const float *bias, int B,
 int esr_conv2d_backward(const float *x, const void *x_split, const float *w, const float *y, const float *dy, int B, int Cin,
                         int H, int W, int Cout, int ksz, int stride, int act, float *dx, float *dw, float *db, void *workspace,
                         size_t workspace_bytes, esr_stream_t stream);
+/* Replaces the same ATen conv2d backward (train_ops.cu, for a ConvLayer of models/submodules.py:159-200) with `flags`: 0 is
+ * esr_conv2d_backward; ESR_DETERMINISTIC sums db and dw from per-block partials in a fixed order (what
+ * torch.backends.cudnn.deterministic asks of cuDNN), with esr_conv2d_workspace_bytes_ex(..., flags) bytes of workspace.  The
+ * opt-in ESR_WGRAD_MMA weight gradient has no deterministic variant: ESR_EUNSUPPORTED. */
+size_t esr_conv2d_workspace_bytes_ex(int B, int Cin, int H, int W, int Cout, int ksz, int stride, int flags);
+int esr_conv2d_backward_ex(const float *x, const void *x_split, const float *w, const float *y, const float *dy, int B, int Cin,
+                           int H, int W, int Cout, int ksz, int stride, int act, float *dx, float *dw, float *db, int flags,
+                           void *workspace, size_t workspace_bytes, esr_stream_t stream);
 /* Bilinear x2 upsampling of `planes` = B*C fp32 planes [H,W] -> [2H,2W] and its backward (dy [2H,2W] -> dx [H,W]):
  * F.interpolate(scale_factor=2, mode='bilinear', align_corners=False) of UpsampleConvLayer (models/submodules.py:290). */
 int esr_upsample2x_forward(const float *x, int planes, int H, int W, float *y, esr_stream_t stream);
@@ -335,6 +363,11 @@ int esr_gru_blend_backward(const float *h, const float *zr, const float *o, cons
 /* loss[0] = mean((pred - target)^2); grad (optional) = grad_scale * 2 (pred - target) / n */
 int esr_mse_loss(const float *pred, const float *target, size_t n, float *loss, float *grad, float grad_scale,
                  esr_stream_t stream);
+/* Replaces the same nn.MSELoss (train_ours_cnt_seq.py:774) with `flags`: 0 is esr_mse_loss; ESR_DETERMINISTIC writes one
+ * partial per block and adds them in block order (workspace: esr_mse_loss_workspace_bytes_ex bytes, 0 without the flag). */
+size_t esr_mse_loss_workspace_bytes_ex(size_t n, int flags);
+int esr_mse_loss_ex(const float *pred, const float *target, size_t n, float *loss, float *grad, float grad_scale, int flags,
+                    void *workspace, size_t workspace_bytes, esr_stream_t stream);
 /* One torch.optim.Adam step over a flat fp32 parameter buffer; max_exp_avg_sq != NULL = amsgrad.  step_counter is a
  * DEVICE int32 holding the number of steps taken so far (0 before the first); the call increments it on the stream and
  * uses the new value for the bias corrections, so the call can sit inside a replayed CUDA graph. */

@@ -1,8 +1,9 @@
 """Times the training iteration (esr_b200.train.train_step: zero_grad, reset_states, L-2 windows forward with carried
 state, summed MSE, one backward, Adam amsgrad) on one GPU and prints one JSON line.  Optional kernel table through
-torch.profiler (CUPTI) with --kernels FILE.
+torch.profiler (CUPTI) with --kernels FILE.  --deterministic sets torch.backends.cudnn.deterministic, as the reference
+trainer's init_seeds does, so the iteration runs the bitwise-reproducible kernels (esr_b200.train.deterministic()).
 
-    python tools/bench_train.py --workload cfg2 --steps 5 --warmup 2 [--kernels gpurun_out/train_kernels.txt]
+    python tools/bench_train.py --workload cfg2 --steps 5 --warmup 2 [--deterministic] [--kernels train_kernels.txt]
 """
 import argparse
 import json
@@ -22,7 +23,9 @@ def main():
     ap.add_argument("--steps", type=int, default=5)
     ap.add_argument("--warmup", type=int, default=2)
     ap.add_argument("--kernels", default=None)
+    ap.add_argument("--deterministic", action="store_true")
     args = ap.parse_args()
+    torch.backends.cudnn.deterministic = args.deterministic
     from esr_b200 import train
     from esr_b200.model import DeepRecurrNet
 
@@ -64,7 +67,9 @@ def main():
     tot = fwd + bwd + step
     out = {"metric": "training LR event-frames/sec (fwd + bwd + Adam)", "value": B * L / (tot * 1e-3), "unit": "frames/s",
            "ms_per_step": tot, "forward_ms": fwd, "backward_ms": bwd, "optimizer_ms": step, "steps": args.steps,
-           "config": {"workload": args.workload, "B": B, "L": L, "hr": [H, W]}, "loss_first": losses[0], "loss_last": losses[-1],
+           "config": {"workload": args.workload, "B": B, "L": L, "hr": [H, W],
+                                                                   "deterministic": args.deterministic},
+           "device": torch.cuda.get_device_name(dev), "loss_first": losses[0], "loss_last": losses[-1],
            "peak_mem_gb": torch.cuda.max_memory_allocated() / 2 ** 30}
     # the same iteration replayed from one CUDA graph
     gstep = train.GraphedTrainStep(net, opt, tuple(frames.shape), dev)
