@@ -272,12 +272,14 @@ int esr_net_get_states(esr_net_t net, float *states, esr_stream_t stream);
 int esr_net_set_states(esr_net_t net, const float *states, esr_stream_t stream);
 
 /* ---------------------------------------------------------------------------------------------
- * The `_ext.dcn_v2_forward` operator (modulated deformable 3x3 convolution), reference layouts in and out.
+ * The `_ext.dcn_v2_forward` operator (modulated deformable convolution), reference layouts in and out.
  * Replaces: models/DCNv2/src/dcn_v2.h:9-27 dcn_v2_forward -> src/cuda/dcn_v2_cuda.cu:20-95 (+ the im2col kernel
  * src/cuda/dcn_v2_im2col_cuda.cu:125-195), as bound by src/vision.cpp:4-8 and called from models/DCNv2/dcn_v2.py:27.
- * input [B,C,H,W], weight [Co,C,3,3], bias [Co], offset [B,dg*18,H,W], mask [B,dg*9,H,W], output [B,Co,H,W]; fp32.
- * Implemented configuration: the one ESR instantiates (C=Co=64, 3x3, stride 1, pad 1, dilation 1, dg=8);
- * anything else returns ESR_EUNSUPPORTED.
+ * input [B,C,H,W], weight [Co,C,k,k], bias [Co], offset [B,dg*2*k*k,Ho,Wo], mask [B,dg*k*k,Ho,Wo], output [B,Co,Ho,Wo];
+ * fp32; Ho = (H + 2*pad - dilation*(k-1) - 1) / stride + 1, likewise Wo.  The kernel, stride, padding and dilation are
+ * square (one value each).  The configuration ESR instantiates (C=Co=64, 3x3, stride 1, pad 1, dilation 1, dg=8) runs on
+ * the wgmma path; any other with C % dg == 0 and Ho, Wo >= 1 on fp32 CUDA-core kernels (csrc/dcn_generic.cu); a bad
+ * geometry returns ESR_EINVAL.  The tensor shapes are not checked here: the caller passes tensors of the sizes above.
  * --------------------------------------------------------------------------------------------- */
 size_t esr_dcn_v2_workspace_bytes(int B, int H, int W);   /* the configuration ESR uses (64 -> 64, 3x3, s1 p1 d1, 8 groups) */
 /* workspace for ANY configuration the reference operator accepts (backward = 1: for esr_dcn_v2_backward).  The configuration

@@ -555,9 +555,10 @@ def dcn_columns64(x, off, m, dg):
     return torch.stack(cols, 2)
 
 
-def _lattice_offsets(g, B, dg, H, W):
+def _lattice_offsets(g, B, dg, H, W, k=3, s=1, p=1, d=1):
     """Offsets (multiples of 1/8, exact in fp32) whose sample positions land on -1, 0, H-1, H (W-1, W), on integers and
-    just inside / outside the border."""
+    just inside / outside the border.  Any square geometry: tap (i, j) of output pixel (y, x) samples around
+    (y*s - p + i*d, x*s - p + j*d); the output is [B, dg*2*k*k, Ho, Wo]."""
     def targets(n, size):
         special = torch.tensor([-1.125, -1.0, -0.875, -0.5, 0.0, 0.125, size - 1.5, size - 1.0, size - 0.875, size - 0.125,
                                 float(size), size + 0.125])
@@ -565,29 +566,41 @@ def _lattice_offsets(g, B, dg, H, W):
         ints = torch.randint(-1, size + 1, (n,), generator=g).float()
         return torch.where(pick, special[torch.randint(0, len(special), (n,), generator=g)], ints)
 
-    off = torch.empty(B, dg, 9, 2, H, W)
-    yy = torch.arange(H).view(H, 1).float()
-    xx = torch.arange(W).view(1, W).float()
-    for kk in range(9):
-        i, j = kk // 3, kk % 3
-        n = B * dg * H * W
-        off[:, :, kk, 0] = targets(n, H).view(B, dg, H, W) - (yy - 1 + i)
-        off[:, :, kk, 1] = targets(n, W).view(B, dg, H, W) - (xx - 1 + j)
-    return off.reshape(B, dg * 18, H, W)
+    Ho, Wo = (H + 2 * p - d * (k - 1) - 1) // s + 1, (W + 2 * p - d * (k - 1) - 1) // s + 1
+    off = torch.empty(B, dg, k * k, 2, Ho, Wo)
+    yy = torch.arange(Ho).view(Ho, 1).float() * s - p
+    xx = torch.arange(Wo).view(1, Wo).float() * s - p
+    for kk in range(k * k):
+        i, j = kk // k, kk % k
+        n = B * dg * Ho * Wo
+        off[:, :, kk, 0] = targets(n, H).view(B, dg, Ho, Wo) - (yy + i * d)
+        off[:, :, kk, 1] = targets(n, W).view(B, dg, Ho, Wo) - (xx + j * d)
+    return off.reshape(B, dg * 2 * k * k, Ho, Wo)
+
+
+# id: (B, H, W, offsets)
+DCN_CASES = {
+    "production_96x32x32": (96, 32, 32, "random"),
+    "lattice_borders": (4, 13, 21, "lattice"),
+    # images smaller than one 16 x 8 / 8 x 16 tile: TMA's out-of-bounds fill supplies most of each box
+    "subtile_1x1": (1, 1, 1, "lattice"),
+    "subtile_2x300": (1, 2, 300, "lattice"),
+    "subtile_300x2": (2, 300, 2, "lattice"),
+    "subtile_7x9": (3, 7, 9, "lattice"),
+}
 
 
 @pytestgpu
-@pytest.mark.parametrize("case", ["production_96x32x32", "lattice_borders"])
+@pytest.mark.parametrize("case", list(DCN_CASES))
 def test_dcn_v2_vs_fp64(dev, case):
     """Forward and the five gradients of `_ext.dcn_v2_forward / backward` (64 -> 64, 8 groups) against float64."""
     from esr_b200 import dcn_v2_ext as ext
     g = torch.Generator().manual_seed(len(case))
     C, G = 64, 8
-    if case == "production_96x32x32":
-        B, H, W = 96, 32, 32
+    B, H, W, offsets = DCN_CASES[case]
+    if offsets == "random":
         off = _rand(g, B, G * 18, H, W, scale=2.0)
     else:
-        B, H, W = 4, 13, 21
         off = _lattice_offsets(g, B, G, H, W)
     x = _rand(g, B, C, H, W)
     w = _rand(g, C, C, 3, 3, scale=1 / 24)
