@@ -113,6 +113,7 @@ SIGNATURES.update({
     "esr_lpips_forward": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p]),
     "esr_render_workspace_bytes": (c_size_t, [c_int, c_int, c_int]),
     "esr_render_event_cnt": (c_int, [c_void_p] + [c_int] * 7 + [c_void_p, c_void_p, c_void_p, c_size_t, c_void_p]),
+    "esr_events_to_columns": (c_int, [c_void_p, c_int, c_i64, c_void_p, c_i64] + [c_void_p] * 5),
 })
 
 SIGNATURES.update({

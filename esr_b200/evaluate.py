@@ -88,27 +88,30 @@ class _Recording:
 
     def encode(self, scaled_out, lr_out, gt_out):
         """Encode the read frames' inp_scaled_cnt into scaled_out [len(frames)], and inp_cnt / gt_cnt of the middle frames
-        into lr_out / gt_out [n_windows] (the encodings of SequenceReader.load_batch)."""
+        into lr_out / gt_out [n_windows] (the encodings of SequenceReader.load_batch).  gt_out None: no ground truth is read."""
         r = self.reader
         (H, W), (kH, kW) = self.res
         ix, iy, _, ip, ioff, imax = r._gather(r.inp_cols, r.index.event_indices, self.frames)
         encodings.encode_frames(ix, iy, ip, ioff, (H, W), (kH, kW), imax, out=scaled_out, sanitised=True)
         lr = encodings.encode_frames(ix, iy, ip, ioff, None, (H, W), imax, sanitised=True)
         lr_out.copy_(lr[torch.as_tensor(np.searchsorted(self.frames, self.mids), device=lr.device)])
+        if gt_out is None:
+            return
         gx, gy, _, gp, goff, gmax = r._gather(r.gt_cols, r.index.gt_event_indices, self.mids)
         encodings.encode_frames(gx, gy, gp, goff, None, (kH, kW), gmax, out=gt_out, sanitised=True)
 
 
-def _steps(model, recs, B, consecutive, chunk, dev):
+def _steps(model, recs, B, consecutive, chunk, dev, need_gt=True):
     """Run one group of recordings (same resolutions) through B lockstep slots.  Yields, per model call, the live
-    (recording, window) pairs with their esr / inp_cnt[mid] / inp_scaled_cnt[mid] / gt[mid] rows and the call's events."""
+    (recording, window) pairs with their esr / inp_cnt[mid] / inp_scaled_cnt[mid] / gt[mid] rows and the call's events.
+    need_gt False (esr_b200.superresolve): the ground-truth stream is neither gathered nor encoded and "gt" is left out."""
     N = recs[0].windows.shape[1]
     (H, W), (kH, kW) = recs[0].res
     cap = max(len(r.frames) for r in recs)
     capw = max(len(r.windows) for r in recs)
     bank = torch.zeros((B * cap + 1, 2, kH, kW), dtype=torch.float32, device=dev)     # last frame: zeros
     lr_bank = torch.empty((B * capw, 2, H, W), dtype=torch.float32, device=dev)
-    gt_bank = torch.empty((B * capw, 2, kH, kW), dtype=torch.float32, device=dev)
+    gt_bank = torch.empty((B * capw, 2, kH, kW), dtype=torch.float32, device=dev) if need_gt else None
     zero = B * cap
     slot_rec, slot_win = [-1] * B, [0] * B
     pending = list(range(len(recs)))
@@ -123,7 +126,7 @@ def _steps(model, recs, B, consecutive, chunk, dev):
         slot_rec[s], slot_win[s] = r, 0
         rec = recs[r]
         rec.encode(bank[s * cap:s * cap + len(rec.frames)], lr_bank[s * capw:s * capw + len(rec.windows)],
-                   gt_bank[s * capw:s * capw + len(rec.windows)])
+                   gt_bank[s * capw:s * capw + len(rec.windows)] if need_gt else None)
         model.reset_sample_states([s])
 
     for s in range(B):
@@ -158,9 +161,11 @@ def _steps(model, recs, B, consecutive, chunk, dev):
         rows = torch.as_tensor([row for _, _, _, row in live], device=dev)
         mid_rows = torch.as_tensor([s * cap + int(np.searchsorted(recs[r].frames, recs[r].mids[w])) for s, r, w, _ in live], device=dev)
         win_rows = torch.as_tensor([s * capw + w for s, _, w, _ in live], device=dev)
-        yield {"rec": [r for _, r, _, _ in live], "win": [w for _, _, w, _ in live], "esr": out.index_select(0, rows),
-               "lr": lr_bank.index_select(0, win_rows), "scaled": bank.index_select(0, mid_rows),
-               "gt": gt_bank.index_select(0, win_rows), "events": ev}
+        st = {"rec": [r for _, r, _, _ in live], "win": [w for _, _, w, _ in live], "esr": out.index_select(0, rows),
+              "lr": lr_bank.index_select(0, win_rows), "scaled": bank.index_select(0, mid_rows), "events": ev}
+        if need_gt:
+            st["gt"] = gt_bank.index_select(0, win_rows)
+        yield st
         for s in range(B):
             r = slot_rec[s]
             if r >= 0:

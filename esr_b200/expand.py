@@ -76,7 +76,7 @@ def _xf_tables(dev):
 
 
 class _ExpandCtx:
-    __slots__ = ("vals", "kind", "dims", "counts", "stats", "stats_host", "event", "parts", "fused_out", "fused_cap", "fused_mcap")
+    __slots__ = ("vals", "kind", "dims", "counts", "stats", "stats_host", "event", "parts", "fused_out", "fused_cap", "fused_mcap", "ev")
 
 
 _PINNED = {}                  # rows -> idle pinned [rows, 4] int64 buffers (cudaHostAlloc per call costs more than the kernels)
@@ -263,7 +263,8 @@ def _emit(ctx, plan, mode, rnd):
 
 
 def expand_finish(ctx, mode):
-    """Phase 2: wait for the statistics, size the output, emit and sort.  Returns CUDA fp32 [B, maxlen, 4].
+    """Phase 2: wait for the statistics, size the output, emit and sort.  Returns CUDA fp32 [B, maxlen, 4] and leaves in ctx.ev
+    (numpy int64 [B]) every sample's number of events: its rows before the padding, 0 for an empty sample (one zero row).
 
     Random mode (mode 1): the reference seeds numpy ONCE per call and draws one continuous stream over all samples in emission
     order (cnt2event.pyx:25,74; event_redistribute.pyx:24) -- also when the batch is processed in 256-sample parts here (the radix
@@ -272,6 +273,7 @@ def expand_finish(ctx, mode):
     dev = ctx.vals.device
     parts = ctx.parts if ctx.parts is not None else [ctx]
     plans = [_host_plan(c) for c in parts]
+    ctx.ev = np.concatenate([np.zeros(c.dims[0], np.int64) if pl is None else pl["ev"] for c, pl in zip(parts, plans)])
     rnds = [None] * len(parts)
     if mode == 1:
         totals = [0 if pl is None else pl["total"] for pl in plans]

@@ -466,6 +466,27 @@ typedef struct {
 int esr_encode_frames_multi(const uint64_t *cols, const esr_frame_desc *desc, int n_frames, int64_t max_len, int H, int W, int kH,
                             int kW, float *out_cnt, float *out_scaled_cnt, esr_stream_t stream);
 
+/* ---------------------------------------------------------------------------------------------
+ * Padded cnt2event rows -> the columns of an event file (esr_b200/superresolve.py).  Completes
+ * dataloader/cython_cnt2event/cnt2event_api.py:25-35 (cnt2eventAPI: its [B, maxlen, 4] rows have no caller in the reference's
+ * scripts) towards the column types of generate_dataset/tools/event_packagers.py:121-224 (xs, ys int16; ts, ps float64).
+ *   rows : fp32 [n_samples, maxlen, 4] = (x, y, t, p) as esr_cnt2event_fused / esr_expand_emit write them (device, 16-byte
+ *          aligned); desc: device table [n_samples]: the first `valid` rows of sample s go to rows [dst, dst + valid) of the
+ *          columns -- the padding and the zero row of an empty sample (valid = 0) are not written -- and its timestamp t32 becomes
+ *          t = t0 + (double)t32 * (t1 - t0): one IEEE subtraction, multiplication and addition, no fused multiply-add, so
+ *          numpy's float64 arithmetic reproduces every bit (BaseDataset.event_formatting, dataloader/base_dataset.py:26-33,
+ *          inverted without its 1e-6);
+ *   max_valid : the largest `valid` (grid sizing; must not exceed maxlen);
+ *   xs, ys, ts, ps : device memory or pinned host memory.  x and y must fit int16: the caller refuses resolutions above 32767.
+ * One launch, no allocation and no synchronisation: graph-capturable.  Negative lengths, max_valid > maxlen, a null or
+ * misaligned pointer return ESR_EINVAL before anything is launched. */
+typedef struct {
+    int64_t valid, dst;
+    double t0, t1;
+} esr_column_desc;
+int esr_events_to_columns(const float *rows, int n_samples, int64_t maxlen, const esr_column_desc *desc, int64_t max_valid,
+                          int16_t *xs, int16_t *ys, double *ts, double *ps, esr_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif
