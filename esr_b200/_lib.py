@@ -79,6 +79,20 @@ SIGNATURES.update({
 })
 
 
+class GlueDesc(ctypes.Structure):
+    """struct esr_glue_desc of include/esr_b200.h"""
+    _fields_ = [
+        ("op", c_int), ("n_img", c_int), ("N", c_int), ("H", c_int), ("W", c_int), ("C", c_int),
+        ("in_", c_void_p), ("in_n_img", c_int), ("in2", c_void_p), ("in2_n_img", c_int), ("idx", c_void_p),
+        ("maps", c_void_p), ("sk", c_void_p), ("ck_in", c_void_p), ("att", c_void_p),
+        ("w0", c_void_p), ("b0", c_void_p), ("w1", c_void_p), ("b1", c_void_p),
+        ("mx", c_void_p), ("ck", c_void_p), ("out", c_void_p), ("out_n_img", c_int),
+    ]
+
+
+SIGNATURES["esr_glue"] = (c_int, [ctypes.POINTER(GlueDesc), c_void_p])
+
+
 SIGNATURES.update({
     "esr_net_param_bytes": (c_size_t, []),
     "esr_net_pack_params": (c_int, [c_void_p, c_void_p, c_void_p]),

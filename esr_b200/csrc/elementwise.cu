@@ -424,3 +424,61 @@ int pack_narrow_weight(const float *w, int cout, int ntaps, float *dst, cudaStre
 }
 
 } // namespace esr
+
+// ---- esr_glue: one launcher of the element-wise glue, as esr_net_forward calls it
+using namespace esr;
+
+static SplitTensor glue_split(const void *p, int n_img, int H, int W, int C)
+{
+    SplitTensor t;
+    t.base = (__nv_bfloat16 *)p; t.n_img = n_img; t.H = H; t.W = W; t.C = C;
+    return t;
+}
+
+extern "C" int esr_glue(const esr_glue_desc *d, esr_stream_t stream)
+{
+    ESR_REQUIRE(d, "esr_glue: null descriptor");
+    const int op = d->op;
+    ESR_REQUIRE(op >= ESR_GLUE_LTC_CAT && op <= ESR_GLUE_COPY_SPLIT, "esr_glue: op %d", op);
+    ESR_REQUIRE(d->n_img > 0 && d->H > 0 && d->W > 0, "esr_glue: n_img=%d H=%d W=%d", d->n_img, d->H, d->W);
+    const bool c64 = op <= ESR_GLUE_ATTN_APPLY;
+    ESR_REQUIRE(c64 ? d->C == 64 : d->C > 0 && d->C % 8 == 0, "esr_glue: op %d has no kernel for C=%d (%s)", op, d->C,
+                c64 ? "64 only" : "a multiple of 8");
+    const int n = d->n_img, N = d->N;
+    const bool needs_in = op != ESR_GLUE_ATTN_MLP, needs_in2 = op == ESR_GLUE_ATTN_APPLY || op == ESR_GLUE_SCALE_AGGREGATE;
+    ESR_REQUIRE(!needs_in || (d->in && d->in_n_img > 0), "esr_glue: op %d: missing input", op);
+    ESR_REQUIRE(!needs_in2 || (d->in2 && d->in2_n_img > 0), "esr_glue: op %d: missing second input", op);
+    ESR_REQUIRE(op != ESR_GLUE_LTC_CAT || (d->idx && d->maps), "esr_glue: ltc_cat needs idx and maps");
+    ESR_REQUIRE(op != ESR_GLUE_ATTN_MLP || (d->mx && d->w0 && d->b0 && d->w1 && d->b1 && d->ck), "esr_glue: attn_mlp: missing mx, weights or ck");
+    ESR_REQUIRE(op != ESR_GLUE_CHAN_MAX || d->mx, "esr_glue: chan_max: missing mx");
+    ESR_REQUIRE(op != ESR_GLUE_ATTN_APPLY || (d->sk && d->ck_in), "esr_glue: attn_apply: missing sk or ck_in");
+    ESR_REQUIRE(op != ESR_GLUE_SCALE_AGGREGATE || (d->att && N > 0), "esr_glue: scale_aggregate: missing att or N=%d", N);
+    const bool split_out = op != ESR_GLUE_CHAN_MAX && op != ESR_GLUE_ATTN_MLP;
+    ESR_REQUIRE(!split_out || d->out, "esr_glue: op %d: missing output", op);
+    ESR_REQUIRE(d->out_n_img >= n, "esr_glue: op %d: %d output images for n_img=%d", op, d->out_n_img, n);
+    // inputs read at the output's own image (no table): they must hold n_img images (n_img * N frames for the aggregation)
+    ESR_REQUIRE(!(op == ESR_GLUE_CHAN_MAX || op == ESR_GLUE_ATTN_APPLY || op == ESR_GLUE_SCALE_AGGREGATE || op == ESR_GLUE_UPSAMPLE2X ||
+                  (op == ESR_GLUE_COPY_SPLIT && !d->idx)) || d->in_n_img >= n,
+                "esr_glue: op %d: input holds %d images for n_img=%d", op, d->in_n_img, n);
+    ESR_REQUIRE(!(op == ESR_GLUE_SCALE_AGGREGATE && !d->idx) || (long long)d->in2_n_img >= (long long)n * N,
+                "esr_glue: scale_aggregate: %d frames for n_img=%d x N=%d", d->in2_n_img, n, N);
+    ESR_REQUIRE(!(op == ESR_GLUE_ATTN_APPLY && !d->idx) || d->in2_n_img >= n, "esr_glue: attn_apply: second input holds %d images for n_img=%d",
+                d->in2_n_img, n);
+    // grid limits: chan_max puts images on grid y, upsample2x output rows on y and images on z
+    ESR_REQUIRE(op != ESR_GLUE_CHAN_MAX || n <= 65535, "esr_glue: chan_max: n_img=%d > 65535", n);
+    ESR_REQUIRE(op != ESR_GLUE_UPSAMPLE2X || (2 * (long long)d->H <= 65535 && n <= 65535), "esr_glue: upsample2x: 2H=%lld or n_img=%d > 65535",
+                2 * (long long)d->H, n);
+
+    cudaStream_t st = (cudaStream_t)stream;
+    const int H = d->H, W = d->W, C = d->C;
+    const SplitTensor in = glue_split(d->in, d->in_n_img, H, W, C), in2 = glue_split(d->in2, d->in2_n_img, H, W, C);
+    switch (op) {
+    case ESR_GLUE_LTC_CAT: return ltc_cat(in, d->maps, d->idx, n, glue_split(d->out, d->out_n_img, H, W, 192), st);
+    case ESR_GLUE_CHAN_MAX: return chan_max(in, n, (float *)d->mx, st);
+    case ESR_GLUE_ATTN_MLP: return attn_mlp((const float *)d->mx, n, d->w0, d->b0, d->w1, d->b1, d->ck, st);
+    case ESR_GLUE_ATTN_APPLY: return attn_apply(in, in2, d->idx, d->sk, d->ck_in, n, glue_split(d->out, d->out_n_img, H, W, 128), st);
+    case ESR_GLUE_SCALE_AGGREGATE: return scale_aggregate(in, in2, d->att, d->idx, n, N, glue_split(d->out, d->out_n_img, H, W, C), st);
+    case ESR_GLUE_UPSAMPLE2X: return upsample2x(in, n, glue_split(d->out, d->out_n_img, 2 * H, 2 * W, C), st);
+    default: return copy_split(in, d->idx, n, glue_split(d->out, d->out_n_img, H, W, C), st);
+    }
+}

@@ -157,3 +157,48 @@ def conv_small(kind, path, x, w, bias, n_img, out=None, out_f32=None, in_img=Non
     _lib.check(L.esr_conv_small(ctypes.byref(d), _lib.stream_ptr()), f"esr_conv_small({kind}, {path})")
     torch.cuda.current_stream().synchronize()
     return out if out is not None else out_f32
+
+
+# esr_glue ops (include/esr_b200.h)
+GLUE_OPS = {"ltc_cat": 0, "chan_max": 1, "attn_mlp": 2, "attn_apply": 3, "scale_aggregate": 4, "upsample2x": 5, "copy_split": 6}
+
+
+def glue(op, n_img, H, W, C, x=None, x2=None, idx=None, N=0, maps=None, sk=None, ck_in=None, att=None, mlp=None, mx=None,
+         ck=None, out=None):
+    """One launcher of the network's element-wise glue (esr_glue) on n_img images of H x W.
+    x, x2, out: Split (their n_img sets the plane stride); idx: int table or None; maps / sk / ck_in / att: fp32 CUDA tensors;
+    mlp = (w0, b0, w1, b1); mx: int32 [*, 64] (chan_max writes it, attn_mlp reads it); ck: fp32 [*, 128] (attn_mlp).
+    The image count of mx (chan_max) or ck (attn_mlp) is passed as the output's."""
+    d = _lib.GlueDesc()
+    d.op, d.n_img, d.N, d.H, d.W, d.C = GLUE_OPS[op], n_img, N, H, W, C
+    keep = []
+
+    def addr(t):
+        if t is None:
+            return None
+        t = t.contiguous()
+        keep.append(t)
+        return t.data_ptr()
+
+    if x is not None:
+        d.in_, d.in_n_img = x.buf.data_ptr(), x.n_img
+    if x2 is not None:
+        d.in2, d.in2_n_img = x2.buf.data_ptr(), x2.n_img
+    if idx is not None:
+        d.idx = addr(idx.to(dtype=torch.int32, device=torch.device("cuda", torch.cuda.current_device())))
+    d.maps, d.sk, d.ck_in, d.att = addr(maps), addr(sk), addr(ck_in), addr(att)
+    if mlp is not None:
+        d.w0, d.b0, d.w1, d.b1 = (addr(t.float()) for t in mlp)
+    if mx is not None:
+        d.mx = mx.data_ptr()
+    if ck is not None:
+        d.ck = ck.data_ptr()
+    if out is not None:
+        d.out, d.out_n_img = out.buf.data_ptr(), out.n_img
+    elif op == "chan_max" and mx is not None:
+        d.out_n_img = mx.shape[0]
+    elif op == "attn_mlp" and ck is not None:
+        d.out_n_img = ck.shape[0]
+    _lib.check(_lib.lib().esr_glue(ctypes.byref(d), _lib.stream_ptr()), f"esr_glue({op})")
+    torch.cuda.current_stream().synchronize()
+    return out

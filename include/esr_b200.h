@@ -215,6 +215,46 @@ size_t esr_conv_small_workspace_bytes(int kind, int path);
 int esr_conv_small(const esr_conv_small_desc *desc, esr_stream_t stream);
 
 /* ---------------------------------------------------------------------------------------------
+ * The element-wise glue of the network, launcher by launcher (for tests and tools; esr_net_forward calls the same launchers).
+ * One call runs one of them, chosen by `op`, on n_img images of H x W.  Split tensors are [2 planes][*_n_img][H][W][C] bf16,
+ * and each one's image count sets its plane stride.  `idx` is the op's int32 index table; NULL = identity where allowed.
+ *   op            reads                                                       writes                                   C
+ *   LTC_CAT       in [*, H, W, 64]; maps fp32 [*, H, W]; idx [n_img][5] =    out [out_n_img, H, W, 192]               64
+ *                 (f0, f1, f2, map0, map1) (required): cat(f0 m0, f1, f2 m1)
+ *   CHAN_MAX      in [>= n_img, H, W, 64]: the per-image channel max          mx int32 [out_n_img, 64], the fp32 max   64
+ *                                                                             as ordered ints (i >= 0 ? i : i ^ 0x7fffffff)
+ *   ATTN_MLP      mx (as CHAN_MAX writes it); w0 [32, 64], b0 [32],           ck fp32 [out_n_img, 128]                 64
+ *                 w1 [128, 32], b1 [128]: sigmoid(w1 relu(w0 max + b0) + b1)
+ *   ATTN_APPLY    in [>= n_img, H, W, 64]; in2 [*, H, W, 64] at image         out [out_n_img, H, W, 128]               64
+ *                 idx[img] (or img); sk fp32 [n_img, H, W, 2]; ck [n_img, 128]:
+ *                 cat(in sk0 ck[:64], in2 sk1 ck[64:])
+ *   SCALE_AGGREGATE  in [>= n_img, H, W, C]; in2 [*, H, W, C] and att fp32   out [out_n_img, H, W, C]                 8k
+ *                 [*, H, W] at frame f = idx[img * N + n] (or img * N + n):
+ *                 in + mean over n < N of in2[f] att[f]
+ *   UPSAMPLE2X    in [>= n_img, H, W, C]: bilinear x2, align_corners=False    out [out_n_img, 2H, 2W, C]               8k
+ *   COPY_SPLIT    in [*, H, W, C] at image idx[img] (or img)                  out [out_n_img, H, W, C]                 8k
+ * ESR_EINVAL before any launch: a missing pointer, a C the op is not written for, n_img, H, W (or N) < 1, too few images in
+ * an output or in an input read without a table, n_img > 65535 for CHAN_MAX and UPSAMPLE2X, 2H > 65535 for UPSAMPLE2X.
+ * --------------------------------------------------------------------------------------------- */
+enum {
+    ESR_GLUE_LTC_CAT = 0, ESR_GLUE_CHAN_MAX, ESR_GLUE_ATTN_MLP, ESR_GLUE_ATTN_APPLY, ESR_GLUE_SCALE_AGGREGATE,
+    ESR_GLUE_UPSAMPLE2X, ESR_GLUE_COPY_SPLIT
+};
+typedef struct esr_glue_desc {
+    int op;
+    int n_img, N, H, W, C;
+    const void *in; int in_n_img;           /* split inputs */
+    const void *in2; int in2_n_img;
+    const int32_t *idx;
+    const float *maps, *sk, *ck_in, *att;   /* fp32 side inputs (ck_in: ATTN_APPLY) */
+    const float *w0, *b0, *w1, *b1;         /* ATTN_MLP */
+    int32_t *mx;                            /* CHAN_MAX output, ATTN_MLP input */
+    float *ck;                              /* ATTN_MLP output */
+    void *out; int out_n_img;               /* split output; out_n_img also counts mx / ck images */
+} esr_glue_desc;
+int esr_glue(const esr_glue_desc *desc, esr_stream_t stream);
+
+/* ---------------------------------------------------------------------------------------------
  * The network: DeepRecurrNet.forward with carried ConvGRU states.
  * Replaces: models/model.py:294-344 (DeepRecurrNet.forward / reset_states), and underneath it
  * models/model.py:20-291, models/submodules.py (ConvLayer, UpsampleConvLayer, ResidualBlock, RecurrentConvLayer,
