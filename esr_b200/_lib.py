@@ -164,6 +164,9 @@ SIGNATURES.update({
 })
 
 
+SIGNATURES["esr_resize_frames_cubic"] = (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p])
+
+
 class ESRError(RuntimeError):
     pass
 

@@ -31,7 +31,7 @@ import random
 import numpy as np
 import torch
 
-from . import _lib, encodings
+from . import _lib, encodings, frames as _frames
 
 MAGIC = b"ESRCOL01"
 HEADER_BYTES = 4096
@@ -61,12 +61,18 @@ class EventStore:
             self.columns[prex] = {c: np.memmap(path, dtype=_DTYPES[c], mode="r", offset=o, shape=(cnt,)) for c, (o, cnt) in cols.items()}
         o, cnt = self.meta["image_ts"]
         self.image_ts = np.memmap(path, dtype=np.float64, mode="r", offset=o, shape=(cnt,)) if cnt else np.zeros(0, np.float64)
+        self.images = None                               # uint8 [n, H, W] or [n, H, W, 3]: the recording's ori_images
+        if "images" in self.meta:
+            o, cnt, shape = self.meta["images"]
+            self.images = np.memmap(path, dtype=np.uint8, mode="r", offset=o, shape=(cnt, *shape))
         self._resident = {}
 
     # ---- writing ---------------------------------------------------------------------------------------------------
     @staticmethod
-    def write(path, columns, sensor_resolution, image_ts=None):
-        """columns: {prefix: {"xs","ys","ts","ps"}} array-likes (cast to the on-disk dtypes of event_packagers.py:129-132)."""
+    def write(path, columns, sensor_resolution, image_ts=None, images=None):
+        """columns: {prefix: {"xs","ys","ts","ps"}} array-likes (cast to the on-disk dtypes of event_packagers.py:129-132).
+        images: optional uint8 frames [n, H, W] (grey) or [n, H, W, 3] (BGR, as the NfS-syn files hold them), one per
+        image timestamp; stored 4 KiB-aligned after image_ts.  Without images the file is laid out as before."""
         image_ts = np.zeros(0, np.float64) if image_ts is None else np.asarray(image_ts, np.float64)
         table, blobs, off = {}, [], HEADER_BYTES
         for prex, cols in columns.items():
@@ -80,14 +86,25 @@ class EventStore:
                 off = (off + a.nbytes + ALIGN - 1) // ALIGN * ALIGN
         meta = {"sensor_resolution": [int(v) for v in sensor_resolution], "columns": table, "image_ts": (off, int(len(image_ts)))}
         blobs.append((off, image_ts))
+        end = off + image_ts.nbytes
+        if images is not None:
+            images = np.ascontiguousarray(images)
+            if images.dtype != np.uint8 or not (images.ndim == 3 or (images.ndim == 4 and images.shape[3] == 3)):
+                raise _lib.ESRError(f"images must be uint8 [n, H, W] or [n, H, W, 3], got {images.dtype} {images.shape}")
+            if len(images) != len(image_ts):
+                raise _lib.ESRError(f"{len(images)} images for {len(image_ts)} image timestamps")
+            off = (end + ALIGN - 1) // ALIGN * ALIGN
+            meta["images"] = (off, int(len(images)), [int(v) for v in images.shape[1:]])
+            blobs.append((off, images))
+            end = off + images.nbytes
         js = json.dumps(meta).encode()
         assert 12 + len(js) <= HEADER_BYTES, "too many columns for the header"
         with open(path, "wb") as f:
             f.write(MAGIC + len(js).to_bytes(4, "little") + js)
             for o, a in blobs:
                 f.seek(o)
-                f.write(a.tobytes())
-            f.truncate(max(off + image_ts.nbytes, HEADER_BYTES))
+                f.write(memoryview(np.ascontiguousarray(a)).cast("B"))
+            f.truncate(max(end, HEADER_BYTES))
         return path
 
     # ---- residency -------------------------------------------------------------------------------------------------
@@ -113,8 +130,17 @@ def convert_hdf5(h5_path, out_path):
             g = f.get(f"{prex}_events")
             if g is not None:
                 cols[prex] = {c: g[c][:] for c in _DTYPES}
-        img_ts = [f[f"ori_images/{name}"].attrs["timestamp"] for name in f["ori_images"]] if "ori_images" in f else []
-        return EventStore.write(out_path, cols, f.attrs["sensor_resolution"].tolist(), img_ts)
+        names = list(f["ori_images"]) if "ori_images" in f else []        # image%09d in name order (h5dataset.py:158-161)
+        img_ts = [f[f"ori_images/{name}"].attrs["timestamp"] for name in names]
+        images = None
+        if names:
+            shape = f[f"ori_images/{names[0]}"].shape
+            if len(shape) == 3 and shape[2] == 1:          # greyscale as [H, W, 1] (event_packagers.py:62-67); cv2.resize drops it
+                shape = shape[:2]
+            images = np.empty((len(names), *shape), np.uint8)
+            for i, name in enumerate(names):
+                images[i] = np.asarray(f[f"ori_images/{name}"][:]).reshape(shape)
+        return EventStore.write(out_path, cols, f.attrs["sensor_resolution"].tolist(), img_ts, images)
 
 
 # ---------------------------------------------------------------------------------------------------------------------
@@ -185,6 +211,16 @@ class WindowIndex:
             idx0 = np.concatenate([[0], idx1[:-1]])
         self.event_indices = np.stack([idx0, idx1], 1).astype(np.int64)
         self.gt_event_indices = self._gt_num(idx0, idx1) if self.need_gt_events else None
+        self.need_gt_frame = bool(config.get("need_gt_frame", False)) and store.images is not None
+        self.need_frame = mode == "frame" and store.images is not None
+        self.gt_image_indices = self._gt_image(idx0, idx1) if self.need_gt_frame else None
+
+    def _gt_image(self, idx0, idx1):
+        """get_gt_frame's image index (h5dataset.py:477-487) of every window: the image timestamps bisected at the input
+        event in the middle of the window, clamped to [0, n - 1]."""
+        ts = np.asarray(self.store.columns[self.inp_prex]["ts"])[(idx0 + idx1) // 2]
+        img_ts = torch.from_numpy(np.ascontiguousarray(self.store.image_ts)).to(self._inp_ts_dev.device)
+        return np.clip(ts_search(img_ts, ts), 0, len(self.store.image_ts) - 1)
 
     def _gt_num(self, idx0, idx1):
         """get_gt_event_indices_num (h5dataset.py:451-475), all windows at once."""
@@ -327,6 +363,8 @@ class SequenceReader:
         self.inp_cols = store.resident(self.index.inp_prex, where)
         self.gt_cols = store.resident(self.index.gt_prex, where) if self.index.need_gt_events else None
         self.inp_sensor_resolution, self.gt_sensor_resolution = self.index.inp_res, self.index.gt_res
+        # the image frames stay in the file; load_batch stages the ones a batch reads (esr_b200.frames)
+        self.images = store.images if (self.index.need_gt_frame or self.index.need_frame) else None
 
     def __len__(self):
         return self.length
@@ -365,6 +403,8 @@ class SequenceReader:
     def load_batch(self, seq_indices):
         """-> the L - num_frame + 1 window dicts of custom_collate for sequences `seq_indices` ('inp_cnt', 'inp_scaled_cnt',
         'gt_cnt' as [B, N, 2, ., .] views of frame banks, 'bank' = the [B, L, 2, ., .] banks for forward_sequence / train_step).
+        A store with images adds 'gt_img' and 'gt_inp_size_img' ([B, L, 1, ., .(, 3)] banks, [B, N, ...] views) with
+        `need_gt_frame`, and 'frame' in mode 'frame', flipped as the events are.
         With augmentation or pauses enabled, the batch consumes the module-level `random` generator as the reference's loader
         would for these sequences in this order; the decisions are kept in `last_decisions`."""
         seq_indices = list(seq_indices)
@@ -385,6 +425,12 @@ class SequenceReader:
         if self.gt_cols is not None:
             gx, gy, _, gp, goff, gmax = self._gather(self.gt_cols, self.index.gt_event_indices, frames, gt_xf, (kH, kW))
             bank["gt_cnt"] = encodings.encode_frames(gx, gy, gp, goff, None, (kH, kW), gmax, sanitised=True).view(B, L, 2, kH, kW)
+        if self.images is not None:
+            flips = gt_xf if gt_xf is not None else np.zeros(B * L, np.int32)
+            pos = np.arange(B * L)
+            gt = [(self.images, self.index.gt_image_indices[frames], pos)] if self.index.need_gt_frame else None
+            fr = [(self.images, frames, pos)] if self.index.need_frame else None
+            bank.update(_frames.batch_frames(gt, fr, flips, B, L, (H, W), (kH, kW), _dev()))
         N = self.num_frame
         return [dict({k: v[:, w:w + N] for k, v in bank.items()}, bank=bank) for w in range(L - N + 1)]
 

@@ -25,7 +25,7 @@ import numpy as np
 import torch
 from torch.utils.data import BatchSampler, ConcatDataset, DistributedSampler, RandomSampler, SequentialSampler
 
-from . import _lib, eventstore
+from . import _lib, eventstore, frames as _frames
 from ._lib import ESRError
 
 EpochPlan = namedtuple("EpochPlan", "batches decisions base_seed")
@@ -126,6 +126,10 @@ class RecordingSequences:
         self.inp_sensor_resolution, self.gt_sensor_resolution = index.inp_res, index.gt_res
         self.inp_cols = self._resident(store, index.inp_prex, where)
         self.gt_cols = self._resident(store, index.gt_prex, where) if index.need_gt_events else None
+        # the image frames (need_gt_frame / mode 'frame' on a store that has them) and each window's gt image
+        self.need_gt_frame, self.need_frame = index.need_gt_frame, index.need_frame
+        self.gt_image_indices = index.gt_image_indices
+        self.images = store.images if (index.need_gt_frame or index.need_frame) else None   # stays in the file
         del index                                         # its float64 ts columns in HBM go with it
 
     @staticmethod
@@ -144,6 +148,8 @@ class RecordingSequences:
         cols = sum(t.numel() * t.element_size() for cs in (self.inp_cols, self.gt_cols or {}) for t in cs.values())
         pinned = any(t.is_pinned() for t in self.inp_cols.values())
         tables = self.event_indices.nbytes + (self.gt_event_indices.nbytes if self.gt_event_indices is not None else 0)
+        if self.gt_image_indices is not None:
+            tables += self.gt_image_indices.nbytes
         return {"host": tables + (cols if pinned else 0), "device": 0 if pinned else cols}
 
 
@@ -189,6 +195,7 @@ class HDF5DataLoaderSequence:
         self._gt_addr = torch.tensor([[d.gt_cols[c].data_ptr() for c in ("xs", "ys", "ps")] for d in recs],
                                      dtype=torch.int64).to(dev) if self._has_gt else None
         self._step = recs[0].step_size
+        self._recs = recs
 
     def __len__(self):
         return len(self.batch_sampler)
@@ -209,6 +216,26 @@ class HDF5DataLoaderSequence:
         for k, batch in enumerate(batches):
             L = self._lengths[batch[0][0]]
             yield self.load(batch, decide(k, len(batch), L))
+
+    def _frames(self, recs, frames, flips, B, L, inp_res, gt_res, dev):
+        """The batch's 'gt_img' / 'gt_inp_size_img' / 'frame' banks (none for recordings without images)."""
+        used = sorted(set(recs.tolist()))
+        has = {r: self._recs[r].images is not None for r in used}
+        if not any(has.values()):
+            return {}
+        if not all(has.values()):
+            raise ESRError(f"a batch mixes recordings with image frames {[r for r in used if has[r]]} and without "
+                           f"{[r for r in used if not has[r]]}: custom_collate cannot stack them")
+        rec_f = np.repeat(recs, L)
+        gt, fr = [], []
+        for r in used:
+            pos = np.flatnonzero(rec_f == r)
+            rs = self._recs[r]
+            if rs.need_gt_frame:
+                gt.append((rs.images, rs.gt_image_indices[frames[pos]], pos))
+            if rs.need_frame:
+                fr.append((rs.images, frames[pos], pos))
+        return _frames.batch_frames(gt or None, fr or None, flips, B, L, inp_res, gt_res, dev)
 
     def load(self, batch, decisions):
         """Window dicts of one batch of (recording, sequence) pairs with draw_decisions' decisions for them."""
@@ -249,5 +276,6 @@ class HDF5DataLoaderSequence:
                                                        kW, 0, 0, _lib.ptr(gt_cnt), None, _lib.stream_ptr()),
                            "esr_encode_frames_multi")
                 bank["gt_cnt"] = gt_cnt
+        bank.update(self._frames(recs, frames, gt_xf, B, L, (H, W), (kH, kW), dev))
         N = self.seqn
         return [dict({k: v[:, w:w + N] for k, v in bank.items()}, bank=bank) for w in range(L - N + 1)]

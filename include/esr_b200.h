@@ -527,6 +527,26 @@ typedef struct {
 int esr_events_to_columns(const float *rows, int n_samples, int64_t maxlen, const esr_column_desc *desc, int64_t max_valid,
                           int16_t *xs, int16_t *ys, double *ts, double *ps, esr_stream_t stream);
 
+/* ---------------------------------------------------------------------------------------------
+ * uint8 frames -> the dataset's fp32 frames (esr_b200/frames.py): BaseDataset.frame_formatting(cv2.resize(augment_frame(img),
+ * dsize, interpolation=cv2.INTER_CUBIC)) of dataloader/h5dataset.py:300-315, 672-685 and base_dataset.py:36-38, many frames
+ * and two target sizes in one launch.  The resize is OpenCV's generic fixed-point bicubic for 8-bit images (A = -0.75,
+ * source position (float)((d + 0.5) * (1 / (dst / src)) - 0.5) in double, coefficients of fp32 polynomials rounded to
+ * nearest-even at 2^11, replicated borders, an exact int32 horizontal pass, then a vertical pass that is an fp32
+ * fused-multiply-add chain rounded to nearest-even for the first floor(oW * C / 8) * 8 elements of a row and
+ * (sum + 2^21) >> 22 for the rest), saturated to uint8; the result is float(u8) / 255 with an IEEE division.
+ *   desc : device table [n]: frame i reads image `src` [H, W(, C)] (pinned host memory or HBM) mirrored by `flips`
+ *          (bit 0: x -> W - 1 - x, bit 1: y -> H - 1 - y, applied to the source before the resize) and writes out0
+ *          [oH0, oW0(, C)] and, unless NULL, out1 [oH1, oW1(, C)], fp32 device memory;
+ *   C    : 1 (grey) or 3 (interleaved colour).  No allocation, no synchronisation. */
+typedef struct {
+    const uint8_t *src;
+    float *out0, *out1;
+    int32_t flips, pad_;
+} esr_frame_resize_desc;
+int esr_resize_frames_cubic(const esr_frame_resize_desc *desc, int n, int H, int W, int C, int oH0, int oW0, int oH1, int oW1,
+                            esr_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif
