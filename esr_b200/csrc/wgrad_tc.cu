@@ -13,7 +13,7 @@
 // One CTA owns (128 M-side channels, 64 N-side channels, a group of <= 3 taps, a slice of the pixel tiles): each of its two
 // consumer warpgroups keeps one 64 x 64 fp32 accumulator per tap in registers (M-side channels [64 w, 64 w + 64)), streams
 // the pixel tiles through a TMA/mbarrier pipeline (the unshifted tensor once per tile, the shifted one once per tap) and adds
-// its partial sums to dw with fp32 atomics at the end.  Which tensor sits on the 128-row M side is chosen per layer:
+// its partial sums to dw with fp32 atomics every WG_FLUSH_TILES tiles and at the end.  Which tensor sits on the 128-row M side is chosen per layer:
 // g (Cout >= 128) or x (Cout == 64 and Cin >= 128); a 64-channel tensor on the M side is loaded twice (rows 64..127
 // ignored).  Warps: 0-7 = MMA + epilogue (two warpgroups), 8 = TMA producer.
 #include "tc_common.cuh"
@@ -24,6 +24,7 @@ namespace esr {
 constexpr int WG_THREADS = 288;
 constexpr int WG_TAPS = 3;                            // taps per CTA (accumulators: 3 x 32 registers per thread)
 constexpr uint32_t WG_TILE = TC_BLOCK_M * 128u;       // one 64-channel x 128-pixel plane: 16 KB
+constexpr int WG_FLUSH_TILES = 32;                   // tiles accumulated in registers between two flushes to dw
 
 struct WgradArgs {
     CUtensorMap gmap, xmap;           // 5-D (C, W, H, img, plane), box (64, TW, TH, 1, 1)
@@ -34,8 +35,9 @@ struct WgradArgs {
     int n_img, H, W, TW, TH, tiles_x, tiles_y, slices;
 };
 
-// DET: instead of the atomics, the CTA of slice s stores its tile to slot s of a.dw = [slices][Cout*Cin*KK] (every CTA of a
-// slice owns distinct elements, and every slice walks at least one tile, so each slot is written in full); sum_slices adds them.
+// DET: instead of the atomics, the CTA of slice s stores its tile to slot s of a.dw = [slices][Cout*Cin*KK] and adds its later
+// flushes there in order (every CTA of a slice owns distinct elements, and every slice walks at least one tile, so each slot is
+// written in full); sum_slices adds them.
 template <bool DET>
 __device__ __forceinline__ void wgrad_tc_body(const WgradArgs &a)
 {
@@ -125,55 +127,70 @@ __device__ __forceinline__ void wgrad_tc_body(const WgradArgs &a)
     for (int j = 0; j < WG_TAPS; ++j)
 #pragma unroll
         for (int i = 0; i < 32; ++i) acc[j][i] = 0.0f;
-    uint32_t gs = 0, gph = 0, xs = 0, xph = 0;
-    for (int t = slice; t < n_tiles; t += a.slices) {
-        mbar_wait(bar_gfull + 8u * gs, gph);
-        const uint32_t gb = once_base + gs * once_bytes;
+    // accumulator fragments -> dw (atomics, or this slice's slot in DET mode: the first flush stores, later ones add in order)
+    const int w = warp & 3;
+    bool first = true;
+    auto flush = [&]() {
 #pragma unroll
         for (int j = 0; j < WG_TAPS; ++j) {
             if (j >= ntap) break;
-            mbar_wait(bar_xfull + 8u * xs, xph);
-            const uint32_t xb = ring_base + xs * tap_bytes;
-            const uint32_t m_hi = (a.a_is_x ? xb : gb) + (uint32_t)wg * WG_TILE, m_lo = m_hi + 2u * WG_TILE;   // this warpgroup's M tile
-            const uint32_t n_hi = a.a_is_x ? gb : xb, n_lo = n_hi + WG_TILE;                                   // N side planes
-            const uint64_t dah = wgmma_desc(m_hi, WG_TILE), dal = wgmma_desc(m_lo, WG_TILE);
-            const uint64_t dbh = wgmma_desc(n_hi, WG_TILE), dbl = wgmma_desc(n_lo, WG_TILE);
-            acc_fence<32>(acc[j]);
-            wgmma_fence();
+            const int tap = tap0 + j;
 #pragma unroll
-            for (int k = 0; k < 8; ++k) {                        // 8 x (K = 16 pixels = 16 rows = 2048 bytes)
-                wgmma_rows<64, 1>(acc[j], dal + 128 * k, dbh + 128 * k);
-                wgmma_rows<64, 1>(acc[j], dah + 128 * k, dbl + 128 * k);
-                wgmma_rows<64, 1>(acc[j], dah + 128 * k, dbh + 128 * k);
-            }
-            wgmma_commit();
-            wgmma_wait<0>();
-            acc_fence<32>(acc[j]);
-            if (lane == 0) mbar_arrive(bar_xempty + 8u * xs);
-            if (++xs == 2) { xs = 0; xph ^= 1u; }
-        }
-        if (lane == 0) mbar_arrive(bar_gempty + 8u * gs);
-        if (++gs == 2) { gs = 0; gph ^= 1u; }
-    }
-    if (slice >= n_tiles) return;
-
-    // ===================== epilogue: accumulator fragments -> fp32 atomics into dw =====================
-    const int w = warp & 3;
-#pragma unroll
-    for (int j = 0; j < WG_TAPS; ++j) {
-        if (j >= ntap) break;
-        const int tap = tap0 + j;
-#pragma unroll
-        for (int i = 0; i < 32; ++i) {
-            const int m = wg * 64 + 16 * w + (lane >> 2) + 8 * ((i >> 1) & 1);   // accumulator row = M-side channel
-            const int nc = n0 + 8 * (i >> 2) + 2 * (lane & 3) + (i & 1);        // column = N-side channel
-            const bool row_ok = (m < 64 || !m_dup) && (m0 + m < m_real);
-            const int co = a.a_is_x ? nc : m0 + m, ci = a.a_is_x ? m0 + m : nc;
-            if (row_ok && co < a.Cout) {
-                if (DET) a.dw[(size_t)slice * a.Cout * a.Cin * a.KK + ((size_t)co * a.Cin + ci) * a.KK + tap] = acc[j][i];
-                else atomicAdd(a.dw + ((size_t)co * a.Cin + ci) * a.KK + tap, acc[j][i]);
+            for (int i = 0; i < 32; ++i) {
+                const int m = wg * 64 + 16 * w + (lane >> 2) + 8 * ((i >> 1) & 1);   // accumulator row = M-side channel
+                const int nc = n0 + 8 * (i >> 2) + 2 * (lane & 3) + (i & 1);        // column = N-side channel
+                const bool row_ok = (m < 64 || !m_dup) && (m0 + m < m_real);
+                const int co = a.a_is_x ? nc : m0 + m, ci = a.a_is_x ? m0 + m : nc;
+                if (row_ok && co < a.Cout) {
+                    if (DET) {
+                        float &d = a.dw[(size_t)slice * a.Cout * a.Cin * a.KK + ((size_t)co * a.Cin + ci) * a.KK + tap];
+                        d = first ? acc[j][i] : d + acc[j][i];
+                    } else {
+                        atomicAdd(a.dw + ((size_t)co * a.Cin + ci) * a.KK + tap, acc[j][i]);
+                    }
+                }
+                acc[j][i] = 0.0f;
             }
         }
+        first = false;
+    };
+    uint32_t gs = 0, gph = 0, xs = 0, xph = 0;
+    // The wgmma accumulation into fp32 drifts with the length of the chain (measured against float64 at cfg4's 672 tiles per
+    // CTA: 6e-4 relative, within 3x of a kernel that drops a cross term), so a CTA hands its sums to dw every WG_FLUSH_TILES
+    // tiles and restarts from zero.
+#pragma unroll 1
+    for (int c0 = slice; c0 < n_tiles; c0 += WG_FLUSH_TILES * a.slices) {
+        const int c1 = min(n_tiles, c0 + WG_FLUSH_TILES * a.slices);
+        for (int t = c0; t < c1; t += a.slices) {
+            mbar_wait(bar_gfull + 8u * gs, gph);
+            const uint32_t gb = once_base + gs * once_bytes;
+#pragma unroll
+            for (int j = 0; j < WG_TAPS; ++j) {
+                if (j >= ntap) break;
+                mbar_wait(bar_xfull + 8u * xs, xph);
+                const uint32_t xb = ring_base + xs * tap_bytes;
+                const uint32_t m_hi = (a.a_is_x ? xb : gb) + (uint32_t)wg * WG_TILE, m_lo = m_hi + 2u * WG_TILE;   // this warpgroup's M tile
+                const uint32_t n_hi = a.a_is_x ? gb : xb, n_lo = n_hi + WG_TILE;                                   // N side planes
+                const uint64_t dah = wgmma_desc(m_hi, WG_TILE), dal = wgmma_desc(m_lo, WG_TILE);
+                const uint64_t dbh = wgmma_desc(n_hi, WG_TILE), dbl = wgmma_desc(n_lo, WG_TILE);
+                acc_fence<32>(acc[j]);
+                wgmma_fence();
+#pragma unroll
+                for (int k = 0; k < 8; ++k) {                        // 8 x (K = 16 pixels = 16 rows = 2048 bytes)
+                    wgmma_rows<64, 1>(acc[j], dal + 128 * k, dbh + 128 * k);
+                    wgmma_rows<64, 1>(acc[j], dah + 128 * k, dbl + 128 * k);
+                    wgmma_rows<64, 1>(acc[j], dah + 128 * k, dbh + 128 * k);
+                }
+                wgmma_commit();
+                wgmma_wait<0>();
+                acc_fence<32>(acc[j]);
+                if (lane == 0) mbar_arrive(bar_xempty + 8u * xs);
+                if (++xs == 2) { xs = 0; xph ^= 1u; }
+            }
+            if (lane == 0) mbar_arrive(bar_gempty + 8u * gs);
+            if (++gs == 2) { gs = 0; gph ^= 1u; }
+        }
+        flush();
     }
 }
 __global__ void __launch_bounds__(WG_THREADS, 1) k_wgrad_tc(const __grid_constant__ WgradArgs a) { wgrad_tc_body<false>(a); }

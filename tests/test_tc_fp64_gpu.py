@@ -523,8 +523,8 @@ def dcn_columns64(x, off, m, dg):
     the sample position (y - 1 + i) + off formed in fp32 first, as the kernels and the reference's CUDA code do."""
     B, C, H, W = x.shape
     cpg = C // dg
-    ys = torch.arange(H, dtype=torch.float32).view(1, 1, H, 1)
-    xs = torch.arange(W, dtype=torch.float32).view(1, 1, 1, W)
+    ys = torch.arange(H, dtype=torch.float32, device=x.device).view(1, 1, H, 1)
+    xs = torch.arange(W, dtype=torch.float32, device=x.device).view(1, 1, 1, W)
     flat = x.reshape(B, C, H * W)
     r = lambda t: t.repeat_interleave(cpg, dim=1)                                         # noqa: E731
     cols = []
