@@ -14,6 +14,10 @@ import torch
 from . import _lib
 
 
+def _ws(nbytes, device):
+    return torch.empty((max(int(nbytes), 256),), dtype=torch.uint8, device=device)
+
+
 def _check_args(op, input, weight, bias, offset, mask, grad_output, kernel_h, kernel_w, stride_h, stride_w, pad_h, pad_w,
                 dilation_h, dilation_w, deformable_group):
     """The checks both operators make before any launch (the CPU-tensor message first, as in the reference).  The kernels
@@ -60,7 +64,7 @@ def dcn_v2_forward(input, weight, bias, offset, mask, kernel_h, kernel_w, stride
     out = torch.empty((B, Co, Ho, Wo), dtype=torch.float32, device=input.device)
     with torch.cuda.device(input.device):
         nbytes = L.esr_dcn_v2_workspace_bytes_ex(B, C, H, W, Co, kernel_h, stride_h, pad_h, dilation_h, deformable_group, 0)
-        ws = torch.empty((max(nbytes, 256),), dtype=torch.uint8, device=input.device)
+        ws = _ws(nbytes, input.device)
         rc = L.esr_dcn_v2_forward(*[_lib.ptr(t) for t in args], B, C, H, W, Co, kernel_h, stride_h, pad_h, dilation_h,
                                   deformable_group, _lib.ptr(out), _lib.ptr(ws), nbytes, _lib.stream_ptr())
     if rc != 0:
@@ -84,7 +88,7 @@ def dcn_v2_backward(input, weight, bias, offset, mask, grad_output, kernel_h, ke
     with torch.cuda.device(input.device):
         nbytes = L.esr_dcn_v2_backward_workspace_bytes_ex(B, C, H, W, Co, kernel_h, stride_h, pad_h, dilation_h, deformable_group,
                                                           flags)
-        ws = torch.empty((max(nbytes, 256),), dtype=torch.uint8, device=input.device)
+        ws = _ws(nbytes, input.device)
         rc = L.esr_dcn_v2_backward_ex(*[_lib.ptr(t) for t in args], B, C, H, W, Co, kernel_h, stride_h, pad_h, dilation_h,
                                       deformable_group, *[_lib.ptr(t) for t in outs], flags, _lib.ptr(ws), nbytes, _lib.stream_ptr())
     if rc != 0:                                                    # ESRError is a RuntimeError, as the reference raises
