@@ -499,6 +499,92 @@ class Adam(torch.optim.Optimizer):
         self.param_groups[0].update(sd["param_groups"][0])
         self.upload_hyper()
 
+    def _offsets(self, named_params):
+        """Flat-buffer offset of every (name, parameter) in `named_params`' order (matched by identity, not by this
+        optimizer's own parameter order)."""
+        at, off = {}, 0
+        for p in self.params:
+            at[id(p)] = off
+            off += p.numel()
+        try:
+            return [at[id(p)] for _, p in named_params]
+        except KeyError:
+            raise _lib.ESRError("Adam: a named parameter is not one this optimizer updates") from None
+
+    def torch_state_dict(self, named_params):
+        """This state in torch.optim.Adam.state_dict()'s layout, parameter index i = named_params[i] (the reference's
+        optimizer sees the model's parameters in its state_dict key order, train_ours_cnt_seq.py:778)."""
+        named_params = list(named_params)
+        shapes = [tuple(p.shape) for _, p in named_params]
+        return to_torch_adam(shapes, self._offsets(named_params), int(self.step_dev.item()), self.exp_avg.cpu(),
+                             self.exp_avg_sq.cpu(), None if self.max_exp_avg_sq is None else self.max_exp_avg_sq.cpu(),
+                             self.param_groups[0])
+
+    def load_torch_state_dict(self, sd, named_params):
+        """Load a torch.optim.Adam.state_dict() (a reference checkpoint's optimizer states) whose parameter index i is
+        named_params[i]."""
+        named_params = list(named_params)
+        shapes = [tuple(p.shape) for _, p in named_params]
+        flat = from_torch_adam(sd, shapes, self._offsets(named_params), self.flat.numel(), self.max_exp_avg_sq is not None)
+        self.step_dev.fill_(flat["step"])
+        self.exp_avg.copy_(flat["exp_avg"])
+        self.exp_avg_sq.copy_(flat["exp_avg_sq"])
+        if self.max_exp_avg_sq is not None:
+            self.max_exp_avg_sq.copy_(flat["max_exp_avg_sq"])
+        self.param_groups[0].update(flat["group"])
+        self.upload_hyper()
+
+
+def to_torch_adam(shapes, offsets, step, exp_avg, exp_avg_sq, max_exp_avg_sq, group):
+    """Flat Adam moments -> torch.optim.Adam.state_dict(): {'state': {i: {'step', 'exp_avg', 'exp_avg_sq'[,
+    'max_exp_avg_sq']}}, 'param_groups': [{..., 'params': [0..n-1]}]}.  Parameter i has shape shapes[i] and starts at
+    offsets[i] of the flat buffers.  No entry per parameter before the first step, as torch's own."""
+    ref = torch.optim.Adam([torch.zeros(1)]).state_dict()["param_groups"][0]
+    g = dict(ref, **{k: v for k, v in group.items() if k != "params"})
+    g["betas"] = tuple(g["betas"])
+    g["params"] = list(range(len(shapes)))
+    state = {}
+    if step > 0:
+        for i, (shp, off) in enumerate(zip(shapes, offsets)):
+            k = math.prod(shp)
+            st = {"step": torch.tensor(float(step)), "exp_avg": exp_avg[off:off + k].reshape(shp).clone(),
+                  "exp_avg_sq": exp_avg_sq[off:off + k].reshape(shp).clone()}
+            if g["amsgrad"]:
+                st["max_exp_avg_sq"] = max_exp_avg_sq[off:off + k].reshape(shp).clone()
+            state[i] = st
+    return {"state": state, "param_groups": [g]}
+
+
+def from_torch_adam(sd, shapes, offsets, n, amsgrad):
+    """torch.optim.Adam.state_dict() -> {'step', 'exp_avg', 'exp_avg_sq', 'max_exp_avg_sq', 'group'} with flat CPU fp32
+    moments of n elements (the inverse of to_torch_adam).  'step' may be a tensor or, from older torch, an int."""
+    if len(sd["param_groups"]) != 1 or len(sd["param_groups"][0]["params"]) != len(shapes):
+        raise _lib.ESRError(f"Adam: the checkpoint's optimizer has {[len(g['params']) for g in sd['param_groups']]} parameters "
+                            f"in its groups; the model has {len(shapes)} in one")
+    out = {"exp_avg": torch.zeros(n), "exp_avg_sq": torch.zeros(n), "max_exp_avg_sq": torch.zeros(n) if amsgrad else None}
+    steps = set()
+    for i, (shp, off) in enumerate(zip(shapes, offsets)):
+        st = sd["state"].get(i)
+        if st is None:
+            steps.add(0)
+            continue
+        k = math.prod(shp)
+        keys = ("exp_avg", "exp_avg_sq", "max_exp_avg_sq") if amsgrad else ("exp_avg", "exp_avg_sq")
+        if amsgrad and "max_exp_avg_sq" not in st:
+            raise _lib.ESRError("Adam: the checkpoint's optimizer ran with amsgrad=False (no max_exp_avg_sq); the config asks "
+                                "for amsgrad=True")
+        for key in keys:
+            t = st[key]
+            if tuple(t.shape) != tuple(shp):
+                raise _lib.ESRError(f"Adam: parameter {i}: {key} has shape {tuple(t.shape)}, the model's is {tuple(shp)}")
+            out[key][off:off + k] = t.detach().reshape(-1).float().cpu()
+        steps.add(int(st["step"]))
+    if len(steps) > 1:
+        raise _lib.ESRError(f"Adam: the checkpoint's parameters were stepped different numbers of times {sorted(steps)}")
+    out["step"] = steps.pop() if steps else 0
+    out["group"] = {k: v for k, v in sd["param_groups"][0].items() if k not in ("params", "amsgrad")}
+    return out
+
 
 def _step_body(model, optimizer, frames, gt, num_frame, all_reduce):
     Wn = frames.shape[1] - num_frame + 1
@@ -526,7 +612,7 @@ def _step_body(model, optimizer, frames, gt, num_frame, all_reduce):
     if all_reduce is not None:
         all_reduce(optimizer.exchange)
     optimizer.step()
-    return loss.detach()
+    return loss.detach(), pred.detach()
 
 
 def _model_num_frame(model, num_frame):
@@ -548,12 +634,15 @@ def train_step(model, optimizer, frames, gt, num_frame=None, all_reduce=None):
     `all_reduce(exchange)` over the flat gradient bucket + the two logging scalars (DDP's role when the model is not
     DDP-wrapped; after it `optimizer.log` holds the rank-reduced last-window MSE and summed loss, which is everything
     train_ours_cnt_seq.py:238-239 + :339 need -- no extra barrier or collective); one Adam step.  Returns the local summed loss."""
-    return _step_body(model, optimizer, frames, gt, _model_num_frame(model, num_frame), all_reduce)
+    return _step_body(model, optimizer, frames, gt, _model_num_frame(model, num_frame), all_reduce)[0]
 
 
 class GraphedTrainStep:
     """train_step captured once into a CUDA graph (forward, backward, all-reduce hook and the Adam kernel) and replayed:
     no Python / launch overhead per iteration.  Shapes are fixed at construction; data is copied into static buffers.
+    `exchanges` is the number of all_reduce calls the captured graph holds (1 with a hook, 0 without).
+    After a replay `pred` holds the iteration's prediction of every window (window-major [(L-N+1)*B, 2, H, W], the static
+    output of the graph; the trainer's images read the last window from it).
     The graph holds the kernels of the mode it was captured in (`deterministic()` or not); replaying it after the mode has
     changed raises ESRError instead of running the other mode's kernels."""
 
@@ -582,12 +671,20 @@ class GraphedTrainStep:
                 optimizer.max_exp_avg_sq.copy_(keep_max)
             optimizer.step_dev.copy_(keep_step)
 
+        calls = [0]
+
+        def counted(flat):
+            calls[0] += 1
+            all_reduce(flat)
+
         err = None
         for attempt in range(2):
+            calls[0] = 0
             try:
                 self.graph = torch.cuda.CUDAGraph()
                 with torch.cuda.graph(self.graph):
-                    self.loss = _step_body(model, optimizer, self.frames, self.gt, num_frame, all_reduce)
+                    self.loss, self.pred = _step_body(model, optimizer, self.frames, self.gt, num_frame,
+                                                      None if all_reduce is None else counted)
                 err = None
                 break
             except Exception as e:                                # noqa: BLE001 -- rethrown below
@@ -596,6 +693,7 @@ class GraphedTrainStep:
         restore()
         if err is not None:
             raise err
+        self.exchanges = calls[0]                                 # all_reduce calls in the graph: each replay issues them
 
     def __call__(self, frames, gt):
         if deterministic() != self.deterministic:
