@@ -165,6 +165,7 @@ SIGNATURES.update({
 
 
 SIGNATURES["esr_resize_frames_cubic"] = (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p])
+SIGNATURES["esr_resize_frames_cubic_u8"] = (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p])
 
 
 class ESRError(RuntimeError):

@@ -37,32 +37,24 @@ __device__ __forceinline__ CubicTaps cubic_taps(int d, int src, double scale)
     return t;
 }
 
-// one thread per output pixel of either target; blockIdx.y = frame
-__global__ void __launch_bounds__(256)
-k_resize_frames_cubic(const esr_frame_resize_desc *__restrict__ desc, int H, int W, int C, int oH0, int oW0, int oH1, int oW1,
-                      double sx0, double sy0, double sx1, double sy1)
+// output pixel q (row-major over oH x oW) of frame `src` mirrored by `flips`: store(q * C + c, u8) for each channel c
+template <typename Store>
+__device__ __forceinline__ void resize_pixel_cubic(const uint8_t *__restrict__ src, int flips, int H, int W, int C, int oW, int q,
+                                                   double sx, double sy, Store store)
 {
-    const esr_frame_resize_desc d = desc[blockIdx.y];
-    const long long p = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-    const long long n0 = (long long)oH0 * oW0;
-    const bool second = p >= n0;
-    if (second && (!d.out1 || p >= n0 + (long long)oH1 * oW1)) return;
-    const int oW = second ? oW1 : oW0;
-    const int q = (int)(second ? p - n0 : p);
     const int oy = q / oW, ox = q - oy * oW;
-    const CubicTaps tx = cubic_taps(ox, W, second ? sx1 : sx0);
-    const CubicTaps ty = cubic_taps(oy, H, second ? sy1 : sy0);
-    float *out = (second ? d.out1 : d.out0) + (long long)q * C;
+    const CubicTaps tx = cubic_taps(ox, W, sx);
+    const CubicTaps ty = cubic_taps(oy, H, sy);
     const int simd_end = oW * C / 8 * 8;       // VResizeCubicVec_32s8u's 8-element steps; the rest of the row is scalar
     int col[4];
 #pragma unroll
-    for (int k = 0; k < 4; ++k) col[k] = (d.flips & 1) ? W - 1 - tx.i[k] : tx.i[k];
+    for (int k = 0; k < 4; ++k) col[k] = (flips & 1) ? W - 1 - tx.i[k] : tx.i[k];
     for (int c = 0; c < C; ++c) {
         int hs[4];
 #pragma unroll
         for (int r = 0; r < 4; ++r) {
-            const int row = (d.flips & 2) ? H - 1 - ty.i[r] : ty.i[r];
-            const uint8_t *s = d.src + ((long long)row * W) * C + c;
+            const int row = (flips & 2) ? H - 1 - ty.i[r] : ty.i[r];
+            const uint8_t *s = src + ((long long)row * W) * C + c;
             int v = 0;
 #pragma unroll
             for (int k = 0; k < 4; ++k) v += (int)s[(long long)col[k] * C] * tx.c[k];
@@ -79,8 +71,35 @@ k_resize_frames_cubic(const esr_frame_resize_desc *__restrict__ desc, int H, int
         } else {
             u = (hs[0] * ty.c[0] + hs[1] * ty.c[1] + hs[2] * ty.c[2] + hs[3] * ty.c[3] + (1 << 21)) >> 22;
         }
-        out[c] = __fdiv_rn((float)min(max(u, 0), 255), 255.f);
+        store((long long)q * C + c, min(max(u, 0), 255));
     }
+}
+
+// one thread per output pixel of either target; blockIdx.y = frame
+__global__ void __launch_bounds__(256)
+k_resize_frames_cubic(const esr_frame_resize_desc *__restrict__ desc, int H, int W, int C, int oH0, int oW0, int oH1, int oW1,
+                      double sx0, double sy0, double sx1, double sy1)
+{
+    const esr_frame_resize_desc d = desc[blockIdx.y];
+    const long long p = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    const long long n0 = (long long)oH0 * oW0;
+    const bool second = p >= n0;
+    if (second && (!d.out1 || p >= n0 + (long long)oH1 * oW1)) return;
+    float *out = second ? d.out1 : d.out0;
+    resize_pixel_cubic(d.src, d.flips, H, W, C, second ? oW1 : oW0, (int)(second ? p - n0 : p), second ? sx1 : sx0,
+                       second ? sy1 : sy0, [out](long long i, int u) { out[i] = __fdiv_rn((float)u, 255.f); });
+}
+
+// the same resize to one target size, storing the saturated uint8 level itself (cv2.resize's output)
+__global__ void __launch_bounds__(256)
+k_resize_frames_cubic_u8(const esr_frame_resize_u8_desc *__restrict__ desc, int H, int W, int C, int oH, int oW, double sx,
+                         double sy)
+{
+    const esr_frame_resize_u8_desc d = desc[blockIdx.y];
+    const long long p = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (p >= (long long)oH * oW) return;
+    uint8_t *out = d.out;
+    resize_pixel_cubic(d.src, d.flips, H, W, C, oW, (int)p, sx, sy, [out](long long i, int u) { out[i] = (uint8_t)u; });
 }
 
 }  // namespace esr
@@ -100,6 +119,21 @@ extern "C" int esr_resize_frames_cubic(const esr_frame_resize_desc *desc, int n,
     const double sx1 = oW1 ? 1.0 / ((double)oW1 / W) : 0.0, sy1 = oH1 ? 1.0 / ((double)oH1 / H) : 0.0;
     esr::k_resize_frames_cubic<<<dim3((unsigned)((total + 255) / 256), (unsigned)n), 256, 0, (cudaStream_t)stream>>>(
         desc, H, W, C, oH0, oW0, oH1, oW1, sx0, sy0, sx1, sy1);
+    ESR_LAUNCH_CHECK();
+    return ESR_OK;
+}
+
+extern "C" int esr_resize_frames_cubic_u8(const esr_frame_resize_u8_desc *desc, int n, int H, int W, int C, int oH, int oW,
+                                          esr_stream_t stream)
+{
+    ESR_REQUIRE(desc && n >= 0 && (C == 1 || C == 3), "esr_resize_frames_cubic_u8: bad arguments");
+    ESR_REQUIRE(H > 0 && W > 0 && oH > 0 && oW > 0, "esr_resize_frames_cubic_u8: bad sizes");
+    ESR_REQUIRE((long long)H * W * C < (1LL << 40) && (long long)oH * oW < (1LL << 31), "esr_resize_frames_cubic_u8: frames too large");
+    ESR_REQUIRE(n <= 65535, "esr_resize_frames_cubic_u8: at most 65535 frames per launch");
+    if (n == 0) return ESR_OK;
+    const double sx = 1.0 / ((double)oW / W), sy = 1.0 / ((double)oH / H);
+    esr::k_resize_frames_cubic_u8<<<dim3((unsigned)(((long long)oH * oW + 255) / 256), (unsigned)n), 256, 0, (cudaStream_t)stream>>>(
+        desc, H, W, C, oH, oW, sx, sy);
     ESR_LAUNCH_CHECK();
     return ESR_OK;
 }

@@ -33,7 +33,11 @@ images per frame.  Here:
 With image_dir, the five images of infer_body (:104-108) are written per evaluated frame as
 image_dir/<recording>/event_img/{lr_event_img, hr_scaled_event_img, hr_bicubic_event_img, hr_esr_event_img (of round(esr)),
 hr_gt_event_img}/{:09d}.png, rendered on the GPU (esr_b200.render) and written by PIL on a worker thread.  The files hold the
-arrays plot_event_cnt returns, not matplotlib's savefig figure; gt_img is not produced because the event store holds no frames.
+arrays plot_event_cnt returns, not matplotlib's savefig figure.  With gt_img=True (the config's need_gt_frame set and every
+store holding image frames) the sixth image of :109 is written too, as image_dir/<recording>/img/gt_img/{:09d}.png: the
+window's middle-frame gt_img as the uint8 array (gt_img * 255).astype('uint8') -- H x W grey or H x W x 3 in the store's
+channel order -- which is cv2.resize's own output, made by one esr_resize_frames_cubic_u8 launch per step from the frames
+WindowIndex.gt_image_indices picks (get_gt_frame's rule).
 """
 import os
 from collections import defaultdict
@@ -42,7 +46,7 @@ from concurrent.futures import ThreadPoolExecutor
 import numpy as np
 import torch
 
-from . import _lib, encodings, metrics, render
+from . import _lib, encodings, frames, metrics, render
 from .eventstore import SequenceReader
 
 METRIC_KEYS = ("esr_l1", "esr_mse", "esr_ssim", "esr_psnr", "bicubic_l1", "bicubic_mse", "bicubic_ssim", "bicubic_psnr",
@@ -174,14 +178,15 @@ def _steps(model, recs, B, consecutive, chunk, dev, need_gt=True):
                     refill(s)
 
 
-def iter_windows(model, stores, dataset_config, batch=4, chunk=8, consecutive=None, lpips=None):
+def iter_windows(model, stores, dataset_config, batch=4, chunk=8, consecutive=None, lpips=None, recordings=None):
     """Evaluate the recordings and yield, per model call, a dict of the evaluated windows: "rec" (index into stores), "win"
     (window index), CUDA tensors "esr", "bicubic", "gt" ([n, 2, kH, kW]), "lr" (inp_cnt[mid]), "scaled"
     (inp_scaled_cnt[mid]), "stats" (CUDA float64 [2, n, 2, 6]: metrics.plane_stats of esr and of bicubic against gt) and
     "events" (the CUDA events around the model call); with lpips (an esr_b200.lpips.LPIPS) also "lpips" (CUDA float64
     [2, n]: esr_lpips and bicubic_lpips).  Nothing in it synchronises the host with the device.
     consecutive: None runs forward_sequence chunks of `chunk` windows when step_size == 1 and the frame-bank path otherwise;
-    False forces the frame-bank path (the two give identical outputs; the tests compare them)."""
+    False forces the frame-bank path (the two give identical outputs; the tests compare them).
+    recordings: an optional list that receives the recordings' window plans (index = "rec")."""
     check_config(dataset_config)
     nf = model._cfg["num_frame"]
     seq = dataset_config["sequence"]
@@ -195,6 +200,8 @@ def iter_windows(model, stores, dataset_config, batch=4, chunk=8, consecutive=No
         raise ValueError("evaluate: forward_sequence chunks need step_size == 1")
     dev = torch.device("cuda", torch.cuda.current_device())
     recs = [_Recording(s, dataset_config, nf) for s in stores]
+    if recordings is not None:
+        recordings[:] = recs
     groups = defaultdict(list)
     for i, r in enumerate(recs):
         groups[r.res].append(i)
@@ -220,16 +227,52 @@ def _save_png(path, arr):
     Image.fromarray(arr).save(path)
 
 
-def evaluate_recordings(model, stores, dataset_config, batch=4, image_dir=None, chunk=8, consecutive=None, lpips=None):
+def check_gt_img(stores, dataset_config, image_dir):
+    """Refuse gt_img=True where there is nothing to write or nothing to write it from."""
+    if image_dir is None:
+        raise _lib.ESRError("evaluate: gt_img needs image_dir (the images are written there)")
+    if not dataset_config.get("need_gt_frame", False):
+        raise _lib.ESRError("evaluate: gt_img needs need_gt_frame: True in the dataset config")
+    bare = [os.path.basename(s.path) for s in stores if s.images is None]
+    if bare:
+        raise _lib.ESRError(f"evaluate: gt_img needs image frames, and the event stores {bare} hold none")
+
+
+def _gt_images(recs, stores, st, dev):
+    """The step's middle-frame gt_img as uint8 host arrays [kH, kW(, 3)], one per evaluated window: per frame shape (grey and
+    colour recordings may share a step) one staging copy and one resize launch."""
+    by_shape = defaultdict(lambda: defaultdict(lambda: ([], [])))
+    for j, (r, w) in enumerate(zip(st["rec"], st["win"])):
+        req = by_shape[stores[r].images.shape[1:]][r]
+        req[0].append(recs[r].reader.index.gt_image_indices[recs[r].mids[w]])
+        req[1].append(j)
+    host = [None] * len(st["rec"])
+    for reqs in by_shape.values():
+        rows = [j for _, pos in reqs.values() for j in pos]
+        local = {j: k for k, j in enumerate(rows)}
+        out, staged = frames.gt_images_u8([(stores[r].images, ix, [local[j] for j in pos]) for r, (ix, pos) in reqs.items()],
+                                          len(rows), recs[st["rec"][0]].res[1], dev)
+        arr = out.cpu().numpy()
+        del staged                                        # read by the launch that .cpu() has waited for
+        for k, j in enumerate(rows):
+            host[j] = arr[k]
+    return host
+
+
+def evaluate_recordings(model, stores, dataset_config, batch=4, image_dir=None, chunk=8, consecutive=None, lpips=None,
+                        gt_img=False):
     """infer_ours_cnt.py infer mode 1 over `stores` (EventStore objects, one per recording; named by the file's basename)
     with the dataset config `dataset_config` (dataloader_config['dataset']).  -> (results_dict, results_mean) laid out as
     the script's (:336-347): results_dict[key][name] = the recording's MetricTracker average, results_mean[key] = the mean
     over recordings, for the keys of METRIC_KEYS (`time` in device milliseconds per window), and of LPIPS_KEYS when
-    `lpips` (an esr_b200.lpips.LPIPS) is given.  chunk, consecutive: as for iter_windows."""
+    `lpips` (an esr_b200.lpips.LPIPS) is given.  chunk, consecutive: as for iter_windows.  gt_img: also write the
+    img/gt_img PNGs under image_dir (see the module docstring); needs need_gt_frame and image frames in every store."""
     params = sum(p.numel() for p in model.parameters()) / 1e6
     names = [os.path.basename(s.path) for s in stores]
     if len(set(names)) != len(names):
         raise ValueError("evaluate_recordings: recordings must have distinct file names (they name the results)")
+    if gt_img:
+        check_gt_img(stores, dataset_config, image_dir)
     per = [defaultdict(list) for _ in stores]             # per recording: key -> [(window, value)]
     pool = ThreadPoolExecutor(max_workers=4) if image_dir is not None else None
     writes = []
@@ -237,9 +280,17 @@ def evaluate_recordings(model, stores, dataset_config, batch=4, image_dir=None, 
         for nm in names:
             for kind in IMAGE_KINDS:
                 os.makedirs(os.path.join(image_dir, nm, "event_img", kind), exist_ok=False)
+            if gt_img:
+                os.makedirs(os.path.join(image_dir, nm, "img", "gt_img"), exist_ok=False)
+    recs = []
     try:
         steps = []
-        for st in iter_windows(model, stores, dataset_config, batch, chunk, consecutive, lpips):
+        for st in iter_windows(model, stores, dataset_config, batch, chunk, consecutive, lpips, recs):
+            if gt_img:
+                g = _gt_images(recs, stores, st, st["esr"].device)
+                for j, (r, w) in enumerate(zip(st["rec"], st["win"])):
+                    writes.append(pool.submit(_save_png, os.path.join(image_dir, names[r], "img", "gt_img", "{:09d}.png".format(w)),
+                                              g[j]))
             if pool is not None:
                 imgs = [render.render_event_cnt(t) for t in (st["lr"], st["scaled"], st["bicubic"], st["esr"].round(), st["gt"])]
                 host = [im.cpu().numpy() for im in imgs]

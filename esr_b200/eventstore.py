@@ -169,6 +169,23 @@ def resolutions(sensor_resolution, scale, ori_scale, need_gt_events):
     return inp_res, [round(i / gd) for i in sensor_resolution], ori_scale, {1: "ori", 2: "down2", 4: "down4", 8: "down8"}[gd]
 
 
+def dataset_length(store, config):
+    """H5Dataset.length (h5dataset.py:163-195) from the host columns alone: the number of windows of the recording."""
+    inp_prex = resolutions(store.sensor_resolution, config["scale"], config["ori_scale"], config.get("need_gt_events", False))[2]
+    inp_ts = store.columns[inp_prex]["ts"]
+    mode, dl = config["mode"], config.get("dataset_length", None)
+    step = config["window"] - config["sliding_window"]
+    if mode == "events":
+        max_length = max(int(len(inp_ts) / step), 0)
+    elif mode == "time":
+        max_length = max(int((float(inp_ts[-1]) - float(inp_ts[0])) / step), 0)
+    elif mode == "frame":
+        max_length = len(store.image_ts) - 1
+    else:
+        raise Exception("Invalid data mode chosen ({})".format(mode))
+    return (dl if dl <= max_length else max_length) if dl is not None else max_length
+
+
 class WindowIndex:
     """The (idx0, idx1) / (gt_idx0, gt_idx1) tables of H5Dataset.set_data_mode (h5dataset.py:163-262)."""
 
@@ -185,17 +202,9 @@ class WindowIndex:
         dev = _dev()
         self._inp_ts_dev = torch.from_numpy(np.ascontiguousarray(inp_ts)).to(dev)
         self._gt_ts_dev = torch.from_numpy(np.ascontiguousarray(store.columns[self.gt_prex]["ts"])).to(dev) if self.need_gt_events else None
-        mode, dl = config["mode"], config.get("dataset_length", None)
+        mode = config["mode"]
         step = self.window - self.sliding_window
-        if mode == "events":
-            max_length = max(int(self.num_events / step), 0)
-        elif mode == "time":
-            max_length = max(int((self.tk - self.t0) / step), 0)
-        elif mode == "frame":
-            max_length = len(store.image_ts) - 1
-        else:
-            raise Exception("Invalid data mode chosen ({})".format(mode))
-        self.length = (dl if dl <= max_length else max_length) if dl is not None else max_length
+        self.length = dataset_length(store, config)
         if self.length == 0:
             raise Exception("Current voxel generation parameters lead to sequence length of zero")
         i = np.arange(self.length, dtype=np.int64)

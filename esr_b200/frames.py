@@ -13,8 +13,9 @@ import torch
 
 from . import _lib
 
-# struct esr_frame_resize_desc of include/esr_b200.h
+# struct esr_frame_resize_desc and esr_frame_resize_u8_desc of include/esr_b200.h
 _DESC = np.dtype([("src", np.uint64), ("out0", np.uint64), ("out1", np.uint64), ("flips", np.int32), ("pad", np.int32)])
+_DESC_U8 = np.dtype([("src", np.uint64), ("out", np.uint64), ("flips", np.int32), ("pad", np.int32)])
 _MAX_LAUNCH = 65535                                     # frames per launch (gridDim.y)
 
 
@@ -33,6 +34,35 @@ def resize_frames(src, flips, out0, out1, shape, size0, size1, dev):
             k = min(_MAX_LAUNCH, n - s)
             _lib.check(_lib.lib().esr_resize_frames_cubic(_lib.ptr(desc[s * _DESC.itemsize:]), k, H, W, C, size0[0], size0[1],
                                                           size1[0], size1[1], _lib.stream_ptr()), "esr_resize_frames_cubic")
+
+
+def resize_frames_u8(src, flips, out, shape, size, dev):
+    """Frame i = uint8 image at address src[i] of `shape` (H, W, C), mirrored by flips[i], resized to `size` into the uint8
+    address out[i]: cv2.resize's own levels, the value resize_frames divides by 255.  All on `dev`."""
+    n = len(src)
+    if n == 0:
+        return
+    d = np.zeros(n, _DESC_U8)
+    d["src"], d["out"], d["flips"] = src, out, np.asarray(flips, np.int32) & 3
+    H, W, C = shape
+    desc = torch.from_numpy(d.view(np.uint8)).to(dev)
+    with torch.cuda.device(dev):
+        for s in range(0, n, _MAX_LAUNCH):
+            k = min(_MAX_LAUNCH, n - s)
+            _lib.check(_lib.lib().esr_resize_frames_cubic_u8(_lib.ptr(desc[s * _DESC_U8.itemsize:]), k, H, W, C, size[0], size[1],
+                                                             _lib.stream_ptr()), "esr_resize_frames_cubic_u8")
+
+
+def gt_images_u8(requests, n, gt_res, dev):
+    """The uint8 gt_img of n window positions, unflipped: requests as stage_frames takes them (images, image index,
+    positions) -> uint8 CUDA tensor [n, H, W(, 3)] at gt_res, one launch."""
+    staged, addr = stage_frames(requests, n, dev)
+    shape = staged.shape[1:]
+    C = shape[2] if len(shape) == 3 else 1
+    out = torch.empty((n, *gt_res) + ((3,) if C == 3 else ()), dtype=torch.uint8, device=dev)
+    rows = np.uint64(out.data_ptr()) + np.arange(n, dtype=np.uint64) * np.uint64(out[0].numel())
+    resize_frames_u8(addr, np.zeros(n, np.int32), rows, (shape[0], shape[1], C), tuple(gt_res), dev)
+    return out, staged
 
 
 def stage_frames(requests, n, dev):

@@ -37,6 +37,15 @@ def read_datalist(path):
     return pd.read_csv(path, header=None).values.flatten().tolist()
 
 
+def open_store(path):
+    """The EventStore of a datalist entry; ESRError when the entry is not one."""
+    try:
+        return eventstore.EventStore(path)
+    except (ESRError, OSError) as e:
+        raise ESRError(f"{path}: datalist entries must be EventStore files (make them from the reference's HDF5 files "
+                       f"with esr_b200.eventstore.convert_hdf5): {e}") from e
+
+
 def make_sampler(total, loader_config, rank=None, world_size=None):
     """The sampler HDF5DataLoaderSequence hands its DataLoader (h5dataloader.py:187-209) over `total` sequences."""
     if loader_config["use_ddp"]:
@@ -168,12 +177,7 @@ class HDF5DataLoaderSequence:
         where = "pinned" if dataloader_config["pin_memory"] else "device"
         recs = []
         for path in read_datalist(dataloader_config["path_to_datalist_txt"]):
-            try:
-                store = eventstore.EventStore(path)
-            except (ESRError, OSError) as e:
-                raise ESRError(f"{path}: datalist entries must be EventStore files (make them from the reference's HDF5 files "
-                               f"with esr_b200.eventstore.convert_hdf5): {e}") from e
-            recs.append(RecordingSequences(store, ds_cfg, where))
+            recs.append(RecordingSequences(open_store(path), ds_cfg, where))
         self.dataset = ConcatDataset(recs)
         self.gt_sensor_resolution = recs[0].gt_sensor_resolution
         self.inp_sensor_resolution = recs[0].inp_sensor_resolution

@@ -131,6 +131,14 @@ class _Plan:
             pass
 
 
+def load_checkpoint(path, weights_only=True):
+    """A checkpoint file on the CPU -> (the loaded object, the model's state_dict): {'model': {'states': ...}} as the
+    reference's trainer and esr_b200.trainer save it (infer_ours_cnt.py:118-127), or a bare state_dict.
+    weights_only=False unpickles anything (the reference's checkpoints may hold numpy scalars): only for trusted files."""
+    cpt = torch.load(path, map_location="cpu", weights_only=weights_only)
+    return cpt, (cpt["model"]["states"] if "model" in cpt else cpt)
+
+
 class DeepRecurrNet(nn.Module):
     def __init__(self, inch=2, basech=16, num_frame=3, norm=None, activation='relu',
                  has_ltc=True, has_gtc=True, gtc_frozen=False,

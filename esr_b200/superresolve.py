@@ -213,7 +213,7 @@ def main(argv=None):
     """python -m esr_b200.superresolve --checkpoint model.pth --config dataset.json --out-dir DIR store [store ...]
     checkpoint: the reference's layout ({'model': {'states': state_dict}, ...}, infer_ours_cnt.py:118-127) or a bare state_dict;
     config: a JSON file holding dataloader_config['dataset'].  Recording `name` is written to DIR/name."""
-    from .model import DeepRecurrNet
+    from .model import DeepRecurrNet, load_checkpoint
     ap = argparse.ArgumentParser(prog="python -m esr_b200.superresolve")
     ap.add_argument("--checkpoint", required=True)
     ap.add_argument("--config", required=True)
@@ -224,9 +224,9 @@ def main(argv=None):
     a = ap.parse_args(argv)
     with open(a.config) as f:
         config = json.load(f)
-    cpt = torch.load(a.checkpoint, map_location="cpu", weights_only=True)
+    _, states = load_checkpoint(a.checkpoint)
     net = DeepRecurrNet(inch=2, basech=8, num_frame=config["sequence"].get("seqn", 3))
-    net.load_state_dict(cpt["model"]["states"] if "model" in cpt else cpt)
+    net.load_state_dict(states)
     net = net.cuda().eval()
     names = [os.path.basename(p) for p in a.stores]
     if len(set(names)) != len(names):

@@ -547,6 +547,18 @@ typedef struct {
 int esr_resize_frames_cubic(const esr_frame_resize_desc *desc, int n, int H, int W, int C, int oH0, int oW0, int oH1, int oW1,
                             esr_stream_t stream);
 
+/* The same resize with cv2.resize's own uint8 output: the saturated level esr_resize_frames_cubic divides by 255, stored as
+ * it is (infer_ours_cnt.py:109 writes (gt_img * 255).astype('uint8'), which is that level: float32(k) / 255 * 255 truncates
+ * back to k for every k in 0..255).  One target size; frame i of desc [n] reads `src` [H, W(, C)] mirrored by `flips` (as
+ * above) and writes out [oH, oW(, C)] uint8 device memory.  No allocation, no synchronisation. */
+typedef struct {
+    const uint8_t *src;
+    uint8_t *out;
+    int32_t flips, pad_;
+} esr_frame_resize_u8_desc;
+int esr_resize_frames_cubic_u8(const esr_frame_resize_u8_desc *desc, int n, int H, int W, int C, int oH, int oW,
+                               esr_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif
