@@ -8,7 +8,8 @@ images per frame.  Here:
   * `window_frames` is the window rule as a pure host function: SequenceDataset's length (h5dataset.py:743-749, with the
     `L >= length` clamp), `step_size` (None means L) and custom_collate's window 0 (h5dataset.py:289-312, asserting
     L >= seqn).  Evaluated window i reads frames i*step .. i*step+N-1; its middle frame is i*step + (N-1)//2.
-  * Only the frames the windows read are encoded (SequenceReader's gather + encode_frames), into per-slot frame banks.
+  * Only the frames the windows read are encoded (through the reader's eventstore.BatchEncoder, as load_batch encodes),
+    into per-slot frame banks; the ground truth only for the windows' middle frames.
   * B slots each hold one recording and advance in lockstep; a slot whose recording ends takes the next one and its
     carried state is zeroed (DeepRecurrNet.reset_sample_states); a slot with nothing left reads zero frames and its outputs
     are dropped.  Every kernel of the plan works per image, so each recording's outputs, metrics and images are bit for bit
@@ -93,16 +94,11 @@ class _Recording:
     def encode(self, scaled_out, lr_out, gt_out):
         """Encode the read frames' inp_scaled_cnt into scaled_out [len(frames)], and inp_cnt / gt_cnt of the middle frames
         into lr_out / gt_out [n_windows] (the encodings of SequenceReader.load_batch).  gt_out None: no ground truth is read."""
-        r = self.reader
-        (H, W), (kH, kW) = self.res
-        ix, iy, _, ip, ioff, imax = r._gather(r.inp_cols, r.index.event_indices, self.frames)
-        encodings.encode_frames(ix, iy, ip, ioff, (H, W), (kH, kW), imax, out=scaled_out, sanitised=True)
-        lr = encodings.encode_frames(ix, iy, ip, ioff, None, (H, W), imax, sanitised=True)
+        enc = self.reader.encoder
+        lr = enc.encode(self.frames, {"inp_cnt": None, "inp_scaled_cnt": scaled_out})["inp_cnt"]
         lr_out.copy_(lr[torch.as_tensor(np.searchsorted(self.frames, self.mids), device=lr.device)])
-        if gt_out is None:
-            return
-        gx, gy, _, gp, goff, gmax = r._gather(r.gt_cols, r.index.gt_event_indices, self.mids)
-        encodings.encode_frames(gx, gy, gp, goff, None, (kH, kW), gmax, out=gt_out, sanitised=True)
+        if gt_out is not None:
+            enc.encode(self.mids, {"gt_cnt": gt_out})
 
 
 def _steps(model, recs, B, consecutive, chunk, dev, need_gt=True):

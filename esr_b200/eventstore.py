@@ -14,16 +14,19 @@ At the GPU pipeline's speed that loader is the limiter.  Here:
     with the ground-truth alignment of `get_gt_event_indices_num` (h5dataset.py:196-262, 451-475).  Every timestamp lookup of
     a table is ONE batched launch of esr_ts_search, which reproduces the reference's bisection (exact hit returns the probed
     index, base_dataset.py:78-91 = binary_search.pyx:17-38) bit for bit.
-  * `SequenceReader` -- SequenceDataset's frame selection (h5dataset.py:729-791) for a BATCH of sequences, with the
-    training loader's event flips (`data_augment`, h5dataset.py:282-288, 652-670) and random pauses (`sequence.pause`,
-    h5dataset.py:769-789): per-frame slices are gathered from the columns by one kernel launch per event stream
-    (esr_gather_events_aug: int16 / float64 -> fp32 SoA + frame offsets, flips and pauses applied in registers) and scattered
-    by esr_b200.encodings.encode_frames into the three frame banks the scripts read, returned in the window layout of
-    HDF5DataLoaderSequence.custom_collate (esr_b200.dataset.collate_sequence's output format) -- no per-frame Python, no
-    per-frame H2D copy.  The random decisions come from `draw_decisions`, which replays the reference's calls on the
-    module-level `random` generator (see there).
-There is no CPU fallback for the indexing / gather: they are C-ABI calls on a CUDA device.
+  * `SequenceReader` -- one recording's SequenceDataset (h5dataset.py:729-791): its window tables on the host and its int16
+    xs / ys and float64 ps columns (12 B per event and stream; never ts) in pinned host memory or HBM.  `load_batch` is
+    SequenceDataset + custom_collate for a BATCH of its sequences, with the training loader's event flips (`data_augment`,
+    h5dataset.py:282-288, 652-670) and random pauses (`sequence.pause`, h5dataset.py:769-789).  The random decisions come
+    from `draw_decisions`, which replays the reference's calls on the module-level `random` generator (see there).
+  * `BatchEncoder` -- the count banks inp_cnt / inp_scaled_cnt / gt_cnt of any frames of a set of readers: one host-to-device
+    copy of the frame descriptors and one esr_encode_frames_multi launch per event stream, flips and pauses applied in
+    registers -- no per-frame Python, no per-frame H2D copy.  A reader's load_batch, the datalist loader
+    (esr_b200.loader) and evaluation (esr_b200.evaluate) all encode through it; the banks come in the window layout of
+    HDF5DataLoaderSequence.custom_collate (esr_b200.dataset.collate_sequence's output format).
+There is no CPU fallback for the indexing / encoding: they are C-ABI calls on a CUDA device.
 """
+import functools
 import json
 import os
 import random
@@ -31,7 +34,7 @@ import random
 import numpy as np
 import torch
 
-from . import _lib, encodings, frames as _frames
+from . import _lib, frames as _frames
 
 MAGIC = b"ESRCOL01"
 HEADER_BYTES = 4096
@@ -109,13 +112,14 @@ class EventStore:
 
     # ---- residency -------------------------------------------------------------------------------------------------
     def resident(self, prex, where="pinned"):
-        """The four columns of `prex` as torch tensors: 'pinned' (page-locked host memory the gather kernel reads through
-        the unified address space, one copy from the page cache), or 'device' (HBM; 20 bytes per event)."""
+        """The xs, ys and ps columns of `prex` (12 bytes per event; no reader reads ts from them) as torch tensors, made once
+        per store: 'pinned' (page-locked host memory esr_encode_frames_multi reads through the unified address space, one
+        copy from the page cache), or 'device' (HBM)."""
         key = (prex, where)
         if key not in self._resident:
             out = {}
-            for c, a in self.columns[prex].items():
-                t = torch.from_numpy(np.ascontiguousarray(a))
+            for c in ("xs", "ys", "ps"):
+                t = torch.from_numpy(np.ascontiguousarray(self.columns[prex][c]))
                 out[c] = t.pin_memory() if where == "pinned" else t.to(_dev())
             self._resident[key] = out
         return self._resident[key]
@@ -199,9 +203,10 @@ class WindowIndex:
         self.num_gt_events = len(store.columns[self.gt_prex]["ts"]) if self.need_gt_events else None
         self.t0, self.tk = float(inp_ts[0]), float(inp_ts[-1])
         self.window, self.sliding_window = config["window"], config["sliding_window"]
+        # the float64 ts columns live in HBM only while the tables are built
         dev = _dev()
-        self._inp_ts_dev = torch.from_numpy(np.ascontiguousarray(inp_ts)).to(dev)
-        self._gt_ts_dev = torch.from_numpy(np.ascontiguousarray(store.columns[self.gt_prex]["ts"])).to(dev) if self.need_gt_events else None
+        inp_ts_dev = torch.from_numpy(np.ascontiguousarray(inp_ts)).to(dev)
+        gt_ts_dev = torch.from_numpy(np.ascontiguousarray(store.columns[self.gt_prex]["ts"])).to(dev) if self.need_gt_events else None
         mode = config["mode"]
         step = self.window - self.sliding_window
         self.length = dataset_length(store, config)
@@ -216,10 +221,10 @@ class WindowIndex:
                 ends = (step * i.astype(np.float64) + self.t0) + self.window
             else:                                                        # compute_frame_indices
                 ends = np.asarray(store.image_ts[:self.length], np.float64)
-            idx1 = np.minimum(ts_search(self._inp_ts_dev, ends), self.num_events - 1)       # find_ts_index
+            idx1 = np.minimum(ts_search(inp_ts_dev, ends), self.num_events - 1)       # find_ts_index
             idx0 = np.concatenate([[0], idx1[:-1]])
         self.event_indices = np.stack([idx0, idx1], 1).astype(np.int64)
-        self.gt_event_indices = self._gt_num(idx0, idx1) if self.need_gt_events else None
+        self.gt_event_indices = self._gt_num(idx0, idx1, gt_ts_dev) if self.need_gt_events else None
         self.need_gt_frame = bool(config.get("need_gt_frame", False)) and store.images is not None
         self.need_frame = mode == "frame" and store.images is not None
         self.gt_image_indices = self._gt_image(idx0, idx1) if self.need_gt_frame else None
@@ -228,14 +233,14 @@ class WindowIndex:
         """get_gt_frame's image index (h5dataset.py:477-487) of every window: the image timestamps bisected at the input
         event in the middle of the window, clamped to [0, n - 1]."""
         ts = np.asarray(self.store.columns[self.inp_prex]["ts"])[(idx0 + idx1) // 2]
-        img_ts = torch.from_numpy(np.ascontiguousarray(self.store.image_ts)).to(self._inp_ts_dev.device)
+        img_ts = torch.from_numpy(np.ascontiguousarray(self.store.image_ts)).to(_dev())
         return np.clip(ts_search(img_ts, ts), 0, len(self.store.image_ts) - 1)
 
-    def _gt_num(self, idx0, idx1):
+    def _gt_num(self, idx0, idx1, gt_ts_dev):
         """get_gt_event_indices_num (h5dataset.py:451-475), all windows at once."""
         n_gt = self.scale ** 2 * (idx1 - idx0)
         t0 = np.asarray(self.store.columns[self.inp_prex]["ts"])[idx0]
-        g0 = ts_search(self._gt_ts_dev, t0)
+        g0 = ts_search(gt_ts_dev, t0)
         g1 = g0 + n_gt
         neg = g0 < 0
         g0 = np.where(neg, 0, g0)
@@ -252,7 +257,7 @@ class WindowIndex:
         return self.length
 
 
-FLIP_X, FLIP_Y, NEGATE_P, PAUSED = 1, 2, 4, 8        # the transform word of esr_gather_events_aug
+FLIP_X, FLIP_Y, NEGATE_P, PAUSED = 1, 2, 4, 8        # the transform word of esr_frame_desc and esr_gather_events_aug
 _EVENT_FLIPS = {"Horizontal": (0, FLIP_X), "Vertical": (1, FLIP_Y), "Polarity": (2, NEGATE_P)}   # name -> (seed offset, bit)
 
 
@@ -346,7 +351,9 @@ def frame_plan(decisions, seq_indices, step_size):
 
 
 class SequenceReader:
-    """Batched SequenceDataset (h5dataset.py:729-791) + custom_collate on the GPU.
+    """One recording's SequenceDataset (h5dataset.py:729-791): the window tables on the host, the xs / ys / ps columns of
+    the input and ground-truth streams resident ('pinned' or 'device'; no ts column), and load_batch, SequenceDataset +
+    custom_collate for a batch of its sequences on the GPU.
 
     With `data_augment` or `sequence.pause` enabled, load_batch draws its random decisions from the module-level `random`
     generator exactly as the reference's DataLoader(num_workers=0) would for the same sequences in the same order
@@ -372,42 +379,26 @@ class SequenceReader:
         self.inp_cols = store.resident(self.index.inp_prex, where)
         self.gt_cols = store.resident(self.index.gt_prex, where) if self.index.need_gt_events else None
         self.inp_sensor_resolution, self.gt_sensor_resolution = self.index.inp_res, self.index.gt_res
-        # the image frames stay in the file; load_batch stages the ones a batch reads (esr_b200.frames)
-        self.images = store.images if (self.index.need_gt_frame or self.index.need_frame) else None
+        # the image frames stay in the file; a batch stages the ones it reads (esr_b200.frames)
+        self.need_gt_frame, self.need_frame = self.index.need_gt_frame, self.index.need_frame
+        self.gt_image_indices = self.index.gt_image_indices
+        self.images = store.images if (self.need_gt_frame or self.need_frame) else None
 
     def __len__(self):
         return self.length
 
-    def _gather(self, cols, table, frames, xform=None, res=None, need_ts=False):
-        """table [len, 2]; frames: flat list of dataset indices; xform: int32 transform word per frame or None, flipping against
-        res = [H, W] -> (xs, ys, ts|None, ps, off) CUDA fp32 SoA + int64 offsets.  A PAUSED frame holds one zero event."""
-        dev = _dev()
-        n = len(frames)
-        lens = table[frames, 1] - table[frames, 0]
-        if xform is not None:
-            lens = np.where(xform & PAUSED, 1, lens)
-        # start [n] | off [n + 1] | xform [n] int32, packed so that one host-to-device copy carries them all
-        host = np.zeros(2 * n + 1 + (n + 1) // 2, dtype=np.int64)
-        host[:n] = table[frames, 0]
-        host[n + 1:2 * n + 1] = np.cumsum(lens)
-        if xform is not None:
-            host[2 * n + 1:].view(np.int32)[:n] = xform
-        total, mx = int(host[2 * n]), int(lens.max(initial=1))
-        d = torch.from_numpy(host).to(dev)
-        off_d = d[n:2 * n + 1]
-        xf_d = d[2 * n + 1:].view(torch.int32)[:n] if xform is not None else None
-        H, W = res if xform is not None else (0, 0)
-        oxs, oys, ops = (torch.empty((max(total, 1),), dtype=torch.float32, device=dev) for _ in range(3))
-        ots = torch.empty((max(total, 1),), dtype=torch.float32, device=dev) if need_ts else None
-        with torch.cuda.device(dev):
-            _lib.check(_lib.lib().esr_gather_events_aug(_lib.ptr(cols["xs"]), _lib.ptr(cols["ys"]), _lib.ptr(cols["ts"]), _lib.ptr(cols["ps"]),
-                                                        _lib.ptr(d), _lib.ptr(off_d), _lib.ptr(xf_d), int(W), int(H), n, mx,
-                                                        _lib.ptr(oxs), _lib.ptr(oys), _lib.ptr(ots), _lib.ptr(ops), _lib.stream_ptr()),
-                       "esr_gather_events_aug")
-        return oxs[:total], oys[:total], (ots[:total] if need_ts else None), ops[:total], off_d, mx
+    @functools.cached_property
+    def encoder(self):
+        """The BatchEncoder of this reader alone, built at first use."""
+        return BatchEncoder([self])
 
-    def frames_of(self, seq_indices):
-        return np.array([i * self.step_size + k for i in seq_indices for k in range(self.L)], dtype=np.int64)
+    def memory_bytes(self):
+        """{'host': pinned column bytes + window tables, 'device': HBM column bytes} this recording holds."""
+        cols = sum(t.numel() * t.element_size() for cs in (self.inp_cols, self.gt_cols or {}) for t in cs.values())
+        pinned = any(t.is_pinned() for t in self.inp_cols.values())
+        idx = self.index
+        tables = sum(t.nbytes for t in (idx.event_indices, idx.gt_event_indices, idx.gt_image_indices) if t is not None)
+        return {"host": tables + (cols if pinned else 0), "device": 0 if pinned else cols}
 
     def load_batch(self, seq_indices):
         """-> the L - num_frame + 1 window dicts of custom_collate for sequences `seq_indices` ('inp_cnt', 'inp_scaled_cnt',
@@ -420,35 +411,141 @@ class SequenceReader:
         for i in seq_indices:
             assert 0 <= i < self.length
         B, L = len(seq_indices), self.L
-        H, W = self.inp_sensor_resolution
-        kH, kW = self.gt_sensor_resolution
         if self.augmented:
-            self.last_decisions = draw_decisions(self.config, B, L)
-            frames, inp_xf, gt_xf = frame_plan(self.last_decisions, seq_indices, self.step_size)
+            self.last_decisions = decisions = draw_decisions(self.config, B, L)
         else:
-            frames, inp_xf, gt_xf = self.frames_of(seq_indices), None, None
-        ix, iy, _, ip, ioff, imax = self._gather(self.inp_cols, self.index.event_indices, frames, inp_xf, (H, W))
-        inp_cnt = encodings.encode_frames(ix, iy, ip, ioff, None, (H, W), imax, sanitised=True).view(B, L, 2, H, W)
-        inp_scaled = encodings.encode_frames(ix, iy, ip, ioff, (H, W), (kH, kW), imax, sanitised=True).view(B, L, 2, kH, kW)
-        bank = {"inp_cnt": inp_cnt, "inp_scaled_cnt": inp_scaled}
-        if self.gt_cols is not None:
-            gx, gy, _, gp, goff, gmax = self._gather(self.gt_cols, self.index.gt_event_indices, frames, gt_xf, (kH, kW))
-            bank["gt_cnt"] = encodings.encode_frames(gx, gy, gp, goff, None, (kH, kW), gmax, sanitised=True).view(B, L, 2, kH, kW)
-        if self.images is not None:
-            flips = gt_xf if gt_xf is not None else np.zeros(B * L, np.int32)
-            pos = np.arange(B * L)
-            gt = [(self.images, self.index.gt_image_indices[frames], pos)] if self.index.need_gt_frame else None
-            fr = [(self.images, frames, pos)] if self.index.need_frame else None
-            bank.update(_frames.batch_frames(gt, fr, flips, B, L, (H, W), (kH, kW), _dev()))
-        N = self.num_frame
-        return [dict({k: v[:, w:w + N] for k, v in bank.items()}, bank=bank) for w in range(L - N + 1)]
+            decisions = {"flips": np.zeros(B, np.int32), "paused": np.zeros((B, L), bool)}
+        frames, inp_xf, gt_xf = frame_plan(decisions, seq_indices, self.step_size)
+        return batch_windows([self], self.encoder, np.zeros(B * L, np.int64), frames, inp_xf, gt_xf, B, L, self.num_frame)
+
+    def _gather(self, cols, n, xform, res):
+        """One frame's device columns [xs, ys, ts, ps] (its events from row 0 on) -> the frame's formatted events [4, n] fp32,
+        transformed by the word xform against res = [H, W]; a PAUSED frame (n = 1) is the zero event."""
+        H, W = res
+        dev = _dev()
+        d = torch.tensor([0, 0, n, xform], dtype=torch.int64, device=dev)        # start | off [2] | xform (int32)
+        out = torch.empty((4, max(n, 1)), dtype=torch.float32, device=dev)
+        with torch.cuda.device(dev):
+            _lib.check(_lib.lib().esr_gather_events_aug(*(_lib.ptr(c) for c in cols), _lib.ptr(d), _lib.ptr(d[1:]),
+                                                        _lib.ptr(d[3:].view(torch.int32)), int(W), int(H), 1, n,
+                                                        *(_lib.ptr(o) for o in out), _lib.stream_ptr()),
+                       "esr_gather_events_aug")
+        return out[:, :n]
 
     def events_of_frame(self, frame, gt=False, xform=None):
         """One frame's formatted events [4, n] fp32 on the GPU = BaseDataset.event_formatting(H5Dataset.get_events(idx0, idx1)),
         with xform (a transform word of FLIP_X | FLIP_Y | NEGATE_P | PAUSED) = event_formatting(augment_event(...)) against the
         stream's sensor resolution, or the zero event of a paused frame."""
-        cols, table = (self.gt_cols, self.index.gt_event_indices) if gt else (self.inp_cols, self.index.event_indices)
-        res = self.gt_sensor_resolution if gt else self.inp_sensor_resolution
-        xf = None if xform is None else np.array([xform], dtype=np.int32)
-        xs, ys, ts, ps, _, _ = self._gather(cols, table, np.array([frame], dtype=np.int64), xf, res, need_ts=True)
-        return torch.stack([xs, ys, ts, ps])
+        idx = self.index
+        prex, table = (idx.gt_prex, idx.gt_event_indices) if gt else (idx.inp_prex, idx.event_indices)
+        a, b = (int(v) for v in table[frame])
+        xf = 0 if xform is None else int(xform)
+        dev = _dev()
+        cols = []
+        for c in ("xs", "ys", "ts", "ps"):
+            host = np.zeros(max(b - a, 1), _DTYPES[c])          # never empty: the kernel takes no null column
+            host[:b - a] = idx.store.columns[prex][c][a:b]
+            cols.append(torch.from_numpy(host).to(dev))
+        return self._gather(cols, 1 if xf & PAUSED else b - a, xf, self.gt_sensor_resolution if gt else self.inp_sensor_resolution)
+
+
+class BatchEncoder:
+    """The count banks of frames drawn from a set of SequenceReaders (H5Dataset.__getitem__'s inp_cnt, inp_scaled_cnt and
+    gt_cnt, h5dataset.py:337-354, 508-528, with SequenceDataset's flips and pauses, :652-670, 769-789): per call one
+    host-to-device copy of the esr_frame_desc table and one esr_encode_frames_multi launch per event stream.  The readers'
+    window tables, joined, and the device tables of their column addresses are built once, here.  The readers come from
+    one dataset config: all of them have ground-truth columns or none."""
+
+    def __init__(self, readers):
+        dev = _dev()
+        self._base = np.cumsum([0] + [len(r.index.event_indices) for r in readers[:-1]]).astype(np.int64)
+        self._res = [(tuple(r.inp_sensor_resolution), tuple(r.gt_sensor_resolution)) for r in readers]
+        self._cols = [(r.inp_cols, r.gt_cols) for r in readers]          # the columns the address tables point into
+
+        def stream(cols, tables):          # -> (joined window tables, device [R, 3] addresses of xs, ys, ps)
+            return (np.concatenate(tables),
+                    torch.tensor([[c[k].data_ptr() for k in ("xs", "ys", "ps")] for c in cols], dtype=torch.int64).to(dev))
+        self._inp = stream([r.inp_cols for r in readers], [r.index.event_indices for r in readers])
+        self._gt = (stream([r.gt_cols for r in readers], [r.index.gt_event_indices for r in readers])
+                    if readers[0].gt_cols is not None else None)
+
+    def encode(self, rows, out, xform=None, rec=None):
+        """Encode F frames.  rows: int64 [F], each frame's row of its reader's window tables; rec: int64 [F], each frame's
+        reader (None: the first); the frames' readers share their resolutions.  xform: int32 [F] transform words (FLIP_X |
+        FLIP_Y | NEGATE_P | PAUSED) or None; PAUSED zeroes the input frame only, the ground truth of a paused frame is its
+        row's events, flipped.  out: {name: CUDA fp32 tensor [F, 2, ., .] to fill, or None for a new one} for any of
+        'inp_cnt', 'inp_scaled_cnt' (which fills 'inp_cnt' too, in a new tensor when not given) and 'gt_cnt'.
+        -> {name: filled bank} in the order inp_cnt, inp_scaled_cnt, gt_cnt."""
+        F = len(rows)
+        rec = np.zeros(F, np.int64) if rec is None else rec
+        xform = np.zeros(F, np.int32) if xform is None else xform
+        (H, W), (kH, kW) = self._res[rec[0] if F else 0]
+        inp, lift, gt = "inp_cnt" in out or "inp_scaled_cnt" in out, "inp_scaled_cnt" in out, "gt_cnt" in out
+        # input descriptors | ground-truth descriptors, each (start, len, rec | xform << 32): one host-to-device copy
+        host = np.empty((inp + gt, F, 3), np.int64)
+        row = self._base[rec] + rows
+        if inp:
+            tab = self._inp[0][row]
+            host[0, :, 0] = tab[:, 0]
+            host[0, :, 1] = np.where(xform & PAUSED, 1, tab[:, 1] - tab[:, 0])
+            host[0, :, 2] = rec | (xform.astype(np.int64) << 32)
+        if gt:
+            tab = self._gt[0][row]
+            host[-1, :, 0] = tab[:, 0]
+            host[-1, :, 1] = tab[:, 1] - tab[:, 0]
+            host[-1, :, 2] = rec | ((xform & ~PAUSED).astype(np.int64) << 32)
+        dev = _dev()
+        desc = torch.from_numpy(host).to(dev)
+        banks = {}
+        for name, on, h, w in (("inp_cnt", inp, H, W), ("inp_scaled_cnt", lift, kH, kW), ("gt_cnt", gt, kH, kW)):
+            if on:
+                t = out.get(name)
+                if t is None:
+                    t = torch.empty((F, 2, h, w), dtype=torch.float32, device=dev)
+                else:
+                    assert t.is_cuda and t.dtype == torch.float32 and t.is_contiguous() and tuple(t.shape) == (F, 2, h, w), name
+                banks[name] = t
+        lib = _lib.lib()
+        with torch.cuda.device(dev):
+            if inp:
+                _lib.check(lib.esr_encode_frames_multi(_lib.ptr(self._inp[1]), _lib.ptr(desc[0]), F, int(host[0, :, 1].max(initial=0)),
+                                                       H, W, kH, kW, _lib.ptr(banks["inp_cnt"]), _lib.ptr(banks.get("inp_scaled_cnt")),
+                                                       _lib.stream_ptr()), "esr_encode_frames_multi")
+            if gt:
+                _lib.check(lib.esr_encode_frames_multi(_lib.ptr(self._gt[1]), _lib.ptr(desc[-1]), F, int(host[-1, :, 1].max(initial=0)),
+                                                       kH, kW, 0, 0, _lib.ptr(banks["gt_cnt"]), None, _lib.stream_ptr()),
+                           "esr_encode_frames_multi")
+        return banks
+
+
+def _image_banks(readers, rec, frames, flips, B, L):
+    """The batch's 'gt_img' / 'gt_inp_size_img' / 'frame' banks for B * L frame positions (rec, frames: each position's
+    reader and dataset index; flips: its transform words), none when the readers hold no image frames."""
+    used = sorted(set(rec.tolist()))
+    has = {r: readers[r].images is not None for r in used}
+    if not any(has.values()):
+        return {}
+    if not all(has.values()):
+        raise _lib.ESRError(f"a batch mixes recordings with image frames {[r for r in used if has[r]]} and without "
+                            f"{[r for r in used if not has[r]]}: custom_collate cannot stack them")
+    gt, fr = [], []
+    for r in used:
+        pos = np.flatnonzero(rec == r)
+        rd = readers[r]
+        if rd.need_gt_frame:
+            gt.append((rd.images, rd.gt_image_indices[frames[pos]], pos))
+        if rd.need_frame:
+            fr.append((rd.images, frames[pos], pos))
+    rd = readers[used[0]]
+    return _frames.batch_frames(gt or None, fr or None, flips, B, L, rd.inp_sensor_resolution, rd.gt_sensor_resolution, _dev())
+
+
+def batch_windows(readers, encoder, rec, frames, inp_xf, gt_xf, B, L, N):
+    """custom_collate's window dicts for B sequences of L frames drawn from `readers` (encoder: their BatchEncoder).
+    rec, frames: int64 [B * L], each frame's reader and dataset index; inp_xf, gt_xf: frame_plan's transform words.
+    -> the L - N + 1 windows: {bank: [B, N, ...] view} plus 'bank' = the [B, L, ...] banks."""
+    out = dict.fromkeys(("inp_cnt", "inp_scaled_cnt") + (("gt_cnt",) if readers[0].gt_cols is not None else ()))
+    bank = {k: v.view(B, L, *v.shape[1:]) for k, v in encoder.encode(frames, out, inp_xf, rec).items()}
+    bank.update(_image_banks(readers, rec, frames, gt_xf, B, L))
+    return [dict({k: v[:, w:w + N] for k, v in bank.items()}, bank=bank) for w in range(L - N + 1)]
+

@@ -105,6 +105,9 @@ def test_sequence_reader_banks(name, where, tmp_path):
     cfg["sequence"] = {"sequence_length": 4, "step_size": 1, "seqn": 3, "pause": {"enabled": False}}
     rd = es.SequenceReader(store, cfg, where=where)
     assert len(rd) == rd.index.length - 4 + 1
+    # no ts column is kept: the reader holds xs / ys / ps only, its window index no device tensor
+    assert all(set(c) == {"xs", "ys", "ps"} for c in (rd.inp_cols, rd.gt_cols) if c is not None)
+    assert not any(isinstance(v, torch.Tensor) for v in vars(rd.index).values())
     seqs = [0, len(rd) - 1]
     wins = rd.load_batch(seqs)
     assert len(wins) == 2 and tuple(wins[0]["inp_scaled_cnt"].shape[:3]) == (2, 3, 2)

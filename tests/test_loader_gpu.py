@@ -1,7 +1,8 @@
 """GPU: the datalist loader (esr_b200.loader.HDF5DataLoaderSequence, esr_encode_frames_multi) against the reference's own
-HDF5DataLoaderSequence (tests/golden/loader_golden.npz) and against SequenceReader.load_batch run per recording and
-concatenated: banks bit for bit from pinned and device-resident columns, batches mixing recordings, more than 65 535 frames in
-one call, and the reference's validation loop body giving identical losses over both paths."""
+HDF5DataLoaderSequence (tests/golden/loader_golden.npz), against SequenceReader.load_batch run per recording and
+concatenated, and against the same frames composed in numpy and encoded by esr_scatter_cnt: banks bit for bit from pinned
+and device-resident columns, batches mixing recordings, more than 65 535 frames in one call, and the reference's
+validation loop body giving identical losses over both paths."""
 import ast
 import os
 import random
@@ -10,7 +11,7 @@ import numpy as np
 import pytest
 import torch
 
-from esr_b200 import eventstore, loader
+from esr_b200 import encodings, eventstore, loader
 from esr_b200.eventstore import EventStore, SequenceReader
 from tests.test_loader import G, RUNS, _epochs
 
@@ -105,6 +106,44 @@ def _random_config(ori_scale, augment, pause):
 SENSORS = [((180, 320), "down4", 4), ((260, 346), "down2", 2)]      # 45 x 80 -> 90 x 160; 130 x 173 -> 260 x 346
 
 
+def _composed(paths, ds_cfg, batch, dec):
+    """The batch's banks [B * L, 2, ., .] composed without esr_encode_frames_multi: numpy slices of the store's columns,
+    augment_event's flips in numpy (W - 1 - x in float32, exact for int16 coordinates; p negated), a paused input frame as
+    the one zero event, then encodings.encode_frames(sanitised=True), which is esr_scatter_cnt with writeback 2."""
+    stores = [EventStore(p) for p in paths]
+    index = [eventstore.WindowIndex(s, ds_cfg) for s in stores]
+    L = dec["paused"].shape[1]
+    frames, _, _ = eventstore.frame_plan(dec, [s for _, s in batch], ds_cfg["sequence"]["step_size"])
+    (H, W), (kH, kW) = index[0].inp_res, index[0].gt_res
+    streams = {"inp": [], "gt": []}                     # per stream: (x, y, p) of every frame
+    for i, f in enumerate(frames):
+        r, flips, paused = batch[i // L][0], int(dec["flips"][i // L]), bool(dec["paused"][i // L, i % L])
+        idx = index[r]
+        for name, prex, table, h, w in (("inp", idx.inp_prex, idx.event_indices, H, W),
+                                        ("gt", idx.gt_prex, idx.gt_event_indices, kH, kW)):
+            a, b = table[f]
+            c = stores[r].columns[prex]
+            x, y, p = (np.asarray(c[k][a:b]).astype(np.float32) for k in ("xs", "ys", "ps"))
+            if name == "inp" and paused:
+                x, y, p = (np.zeros(1, np.float32) for _ in range(3))
+            else:
+                if flips & eventstore.FLIP_X:
+                    x = np.float32(w - 1) - x
+                if flips & eventstore.FLIP_Y:
+                    y = np.float32(h - 1) - y
+                if flips & eventstore.NEGATE_P:
+                    p = -p
+            streams[name].append((x, y, p))
+    dev = {}
+    for name, evs in streams.items():
+        off = np.cumsum([0] + [len(e[0]) for e in evs])
+        dev[name] = [torch.from_numpy(np.concatenate([e[k] for e in evs])).to(DEV) for k in range(3)]
+        dev[name].append(torch.from_numpy(off).to(DEV))
+    return {"inp_cnt": encodings.encode_frames(*dev["inp"], None, (H, W), sanitised=True),
+            "inp_scaled_cnt": encodings.encode_frames(*dev["inp"], (H, W), (kH, kW), sanitised=True),
+            "gt_cnt": encodings.encode_frames(*dev["gt"], None, (kH, kW), sanitised=True)}
+
+
 @pytest.mark.parametrize("mode", ["augment_pause", "pause", "plain"])
 @pytest.mark.parametrize("sensor", SENSORS, ids=["45x80", "173w"])
 def test_multi_recording_banks_equal_per_recording_load_batch(tmp_path, sensor, mode):
@@ -143,9 +182,11 @@ def test_multi_recording_banks_equal_per_recording_load_batch(tmp_path, sensor, 
             assert dec["paused"].any() and not dec["paused"].all()
         if mode == "augment_pause":
             assert len(set(dec["flips"].tolist())) > 2
+        composed = _composed(paths, ds_cfg, batch, dec)
         for key in BANKS:
             want = torch.cat([p[0]["bank"][key] for p in parts])[inv]
             assert torch.equal(got[0]["bank"][key], want), (where, key)
+            assert torch.equal(want.reshape(composed[key].shape), composed[key]), (where, key)
             assert want.abs().sum() > 0
             for w in range(len(got)):
                 assert torch.equal(got[w][key], want[:, w:w + 3])
