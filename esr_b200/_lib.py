@@ -68,7 +68,6 @@ class ConvSmallDesc(ctypes.Structure):
         ("w", c_void_p), ("bias", c_void_p), ("w_head", c_void_p), ("b_head", c_void_p), ("n_img", c_int),
         ("out", c_void_p), ("out_n_img", c_int), ("out_f32", c_void_p),
         ("crop_top", c_int), ("crop_left", c_int), ("out_H", c_int), ("out_W", c_int),
-        ("agg_feats", c_void_p), ("agg_n_img", c_int), ("agg_att", c_void_p), ("agg_idx", c_void_p), ("agg_N", c_int),
         ("workspace", c_void_p), ("workspace_bytes", c_size_t),
     ]
 

@@ -1,17 +1,11 @@
 // capi.cu -- error reporting, device info and library-level entry points of libesr_b200.so
 #include "common.cuh"
-#include <cstdlib>
 #include <string>
 
 namespace esr {
 
 static thread_local std::string t_err;
 std::atomic<long long> g_launches{0};
-bool pdl_enabled()
-{
-    static const bool on = getenv("ESR_NO_PDL") == nullptr;
-    return on;
-}
 
 void set_error(const char *fmt, ...)
 {

@@ -50,13 +50,12 @@ inline void count_launch(int n = 1) { g_launches.fetch_add(n, std::memory_order_
 // current one has executed `griddepcontrol.launch_dependents` (first instruction of our kernels): its CTAs take over SMs as
 // they free up and run their prologue, then block in `griddepcontrol.wait` until the predecessor grid has COMPLETED and its
 // memory is visible.  Rules kept by every kernel launched through launch_pdl(): no global-memory access of any kind before
-// PDL_WAIT().  Works inside stream capture (the edge becomes a programmatic graph dependency).  ESR_NO_PDL=1: plain launches.
+// PDL_WAIT().  Works inside stream capture (the edge becomes a programmatic graph dependency).
 // ---------------------------------------------------------------------------------------------
 #ifdef __CUDACC__
 #define PDL_LAUNCH_DEPENDENTS() asm volatile("griddepcontrol.launch_dependents;" ::: "memory")
 #define PDL_WAIT() asm volatile("griddepcontrol.wait;" ::: "memory")
 #endif
-bool pdl_enabled();
 template <typename... KArgs, typename... Args>
 static inline cudaError_t launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t st, Args &&...args)
 {
@@ -65,7 +64,7 @@ static inline cudaError_t launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 b
     cudaLaunchAttribute at[1];
     at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
     at[0].val.programmaticStreamSerializationAllowed = 1;
-    cfg.attrs = at; cfg.numAttrs = pdl_enabled() ? 1 : 0;
+    cfg.attrs = at; cfg.numAttrs = 1;
     return cudaLaunchKernelEx(&cfg, kernel, static_cast<KArgs>(args)...);
 }
 

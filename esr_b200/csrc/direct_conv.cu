@@ -321,11 +321,12 @@ struct SmallKind {
     int dk;        // DirectKind of paths 0 and 1 (-1: narrow only)
     int paths;     // bit p: path p runs this kind in the plan
 };
+// indexed by ESR_CONV_SMALL_*; 8 and 9 are unassigned (no path runs them)
 const SmallKind SMALL_KINDS[] = {
     {8, 16, 9, 2, false, DK_HEAD_ENC0, 3}, {16, 32, 9, 2, false, DK_ENC1, 3}, {32, 64, 9, 2, false, DK_ENC2, 3},
-    {32, 1, 9, 1, false, DK_ATT32, 7},     {16, 1, 9, 1, false, DK_ATT16, 7}, {32, 16, 9, 1, true, DK_RECON1, 3},
-    {16, 8, 9, 1, true, DK_RECON2, 3},     {8, 2, 9, 1, false, DK_TAIL, 7},   {64, 1, 9, 1, false, -1, 4},
-    {64, 1, 9, 1, false, -1, 4},           {64, 2, 1, 1, false, -1, 4},
+    {32, 1, 9, 1, false, DK_ATT32, 3},     {16, 1, 9, 1, false, DK_ATT16, 3}, {32, 16, 9, 1, true, DK_RECON1, 3},
+    {16, 8, 9, 1, true, DK_RECON2, 3},     {8, 2, 9, 1, false, DK_TAIL, 3},   {},
+    {},                                    {64, 2, 1, 1, false, -1, 4},
 };
 constexpr int N_SMALL_KINDS = (int)(sizeof(SMALL_KINDS) / sizeof(SMALL_KINDS[0]));
 bool small_ok(int kind, int path) { return kind >= 0 && kind < N_SMALL_KINDS && path >= 0 && path <= 2 && (SMALL_KINDS[kind].paths >> path & 1); }
@@ -365,15 +366,6 @@ extern "C" int esr_conv_small(const esr_conv_small_desc *d, esr_stream_t stream)
     ESR_REQUIRE(split_out ? d->out && d->out_n_img >= d->n_img : d->out_f32 != nullptr, "esr_conv_small: missing output");
     ESR_REQUIRE(head || (d->pad_top | d->pad_bottom | d->pad_left | d->pad_right) == 0, "esr_conv_small: pads are HEAD_ENC0's");
     ESR_REQUIRE(d->pad_top >= 0 && d->pad_bottom >= 0 && d->pad_left >= 0 && d->pad_right >= 0, "esr_conv_small: negative pad");
-    if (d->agg_feats && (d->path != 0 || !k.ups)) {
-        set_error("esr_conv_small: scale aggregation is fused into the mma decoder kernels only");
-        return ESR_EUNSUPPORTED;
-    }
-    ESR_REQUIRE(!d->agg_feats || (d->agg_att && d->agg_N > 0 && d->agg_n_img > 0), "esr_conv_small: agg_att / agg_N / agg_n_img");
-    if (tail && d->path == 2 && d->in_img) {
-        set_error("esr_conv_small: the narrow tail kernel reads images in order");
-        return ESR_EUNSUPPORTED;
-    }
     const int Hc = d->H_in + d->pad_top + d->pad_bottom, Wc = d->W_in + d->pad_left + d->pad_right;
     const int Hout = k.ups ? 2 * Hc : (k.stride == 2 ? (Hc - 1) / 2 + 1 : Hc);
     const int Wout = k.ups ? 2 * Wc : (k.stride == 2 ? (Wc - 1) / 2 + 1 : Wc);
@@ -395,7 +387,6 @@ extern "C" int esr_conv_small(const esr_conv_small_desc *d, esr_stream_t stream)
     if (d->path == 2) {
         SplitTensor x;
         x.base = (__nv_bfloat16 *)d->in; x.n_img = d->in_n_img; x.H = d->H_in; x.W = d->W_in; x.C = k.cin;
-        if (tail) return conv_narrow_tail(x, (const float *)ws, d->bias, d->n_img, d->out_f32, d->crop_top, d->crop_left, d->out_H, d->out_W, st);
         return conv_narrow(x, d->in_img, (const float *)ws, d->bias, k.cout, k.ntaps, d->n_img, d->out_f32, st);
     }
     DirectArgs a;
@@ -414,10 +405,6 @@ extern "C" int esr_conv_small(const esr_conv_small_desc *d, esr_stream_t stream)
     } else {
         a.out_f32 = d->out_f32;
         if (tail) { a.crop_top = d->crop_top; a.crop_left = d->crop_left; a.out_H = d->out_H; a.out_W = d->out_W; }
-    }
-    if (d->agg_feats) {
-        a.agg_feats = (const __nv_bfloat16 *)d->agg_feats; a.agg_plane = (size_t)d->agg_n_img * d->H_in * d->W_in * k.cin;
-        a.agg_att = d->agg_att; a.agg_idx = d->agg_idx; a.agg_N = d->agg_N;
     }
     if (d->path == 1) return conv_direct_choice((DirectKind)k.dk, a, true, st);
     rc = conv_mma((DirectKind)k.dk, a, st);

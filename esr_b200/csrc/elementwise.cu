@@ -297,19 +297,17 @@ int copy_split(const SplitTensor &src, const int *src_img, int n_img, const Spli
 } // namespace esr
 
 // ------------------------------------------------------------------------------------------------
-// Narrow-output convolutions of a 64-channel split tensor: Cout = 1 or 2, 3x3 (pad 1) or 1x1, sigmoid -- pred_map[1]
-// (models/model.py:59-60), attens[0] (:193) and the spatial-attention kernel (:183).  On the tensor cores these layers pad
-// N to 16 and move a full 128 x 64 A tile per tap for 1-2 useful columns (41 / 22 / 19 us per cfg2 step, 1.2 TB/s); they are
-// reads of an L2-resident tensor with 576 MACs per pixel, so plain fp32 FMAs do: 8 lanes per pixel, 8 channels (16 B hi + 16 B lo)
-// each, 3 shuffles to reduce.  fp32 products of the exact hi + lo values (no operand split needed).
+// Narrow-output convolution of a 64-channel split tensor on CUDA cores: the spatial-attention kernel (models/model.py:183),
+// 1x1, Cout = 2, sigmoid.  On the tensor cores it pads N to 16 and moves a full 128 x 64 A tile for 2 useful columns (19 us per
+// cfg2 step, 1.2 TB/s); it is a read of an L2-resident tensor, so plain fp32 FMAs do: 8 lanes per pixel, 8 channels (16 B hi +
+// 16 B lo) each, 3 shuffles to reduce.  fp32 products of the exact hi + lo values (no operand split needed).
 // ------------------------------------------------------------------------------------------------
 namespace esr {
 
-template <int CIN, int COUT, int TAPS, int ACT, int NCHW>
+template <int CIN, int COUT, int TAPS>
 __global__ void __launch_bounds__(256)
 k_conv_narrow(const __nv_bfloat16 *__restrict__ x, size_t plane, const int *__restrict__ src_img, const float *__restrict__ w /*[TAPS][CIN][COUT]*/,
-              const float *__restrict__ bias, int n_img, int H, int W, float *__restrict__ out, int crop_top, int crop_left, int out_H,
-              int out_W)
+              const float *__restrict__ bias, int n_img, int H, int W, float *__restrict__ out)
 {
     PDL_LAUNCH_DEPENDENTS();
     PDL_WAIT();
@@ -329,7 +327,7 @@ k_conv_narrow(const __nv_bfloat16 *__restrict__ x, size_t plane, const int *__re
 #pragma unroll
     for (int c = 0; c < COUT; ++c) acc[c] = 0.0f;
     // branch-free taps: out-of-image neighbours read a clamped (valid) address and are zeroed, so all 2 x TAPS loads of a thread are
-    // independent and issue back to back (the first version's per-tap `if` serialised load -> use -> load: 51 us for pred_map[1])
+    // independent and issue back to back
     uint4 hv[TAPS], lv[TAPS];
 #pragma unroll
     for (int t = 0; t < TAPS; ++t) {
@@ -363,27 +361,17 @@ k_conv_narrow(const __nv_bfloat16 *__restrict__ x, size_t plane, const int *__re
     }
     if (valid && lc == 0) {
 #pragma unroll
-        for (int c = 0; c < COUT; ++c) {
-            const float v = acc[c] + bias[c];
-            const float r = ACT == ACT_SIGMOID ? fast_sigmoid(v) : (ACT == ACT_RELU ? fmaxf(v, 0.0f) : v);
-            if (NCHW) {
-                const int oy = y - crop_top, ox = xx - crop_left;
-                if (oy >= 0 && oy < out_H && ox >= 0 && ox < out_W) out[(((size_t)img * COUT + c) * out_H + oy) * out_W + ox] = r;
-            } else {
-                out[(((size_t)img * H + y) * W + xx) * COUT + c] = r;
-            }
-        }
+        for (int c = 0; c < COUT; ++c) out[(((size_t)img * H + y) * W + xx) * COUT + c] = fast_sigmoid(acc[c] + bias[c]);
     }
 }
 
-template <int CIN, int COUT, int TAPS, int ACT, int NCHW>
-static int launch_narrow(const SplitTensor &x, const int *src_img, const float *w, const float *bias, int n_img, float *out, int crop_top,
-                         int crop_left, int out_H, int out_W, cudaStream_t st)
+template <int CIN, int COUT, int TAPS>
+static int launch_narrow(const SplitTensor &x, const int *src_img, const float *w, const float *bias, int n_img, float *out, cudaStream_t st)
 {
     constexpr int TH = (256 / (CIN / 8)) / 8;
     const dim3 grid((unsigned)(n_img * ((x.W + 7) / 8) * ((x.H + TH - 1) / TH)));
-    ESR_CUDA_CHECK(launch_pdl(k_conv_narrow<CIN, COUT, TAPS, ACT, NCHW>, grid, dim3(256), 0, st, x.base, x.plane(), src_img, w, bias, n_img, x.H,
-                              x.W, out, crop_top, crop_left, out_H, out_W));
+    ESR_CUDA_CHECK(launch_pdl(k_conv_narrow<CIN, COUT, TAPS>, grid, dim3(256), 0, st, x.base, x.plane(), src_img, w, bias, n_img, x.H,
+                              x.W, out));
     esr::count_launch();
     return ESR_OK;
 }
@@ -391,20 +379,9 @@ static int launch_narrow(const SplitTensor &x, const int *src_img, const float *
 int conv_narrow(const SplitTensor &x, const int *src_img, const float *w, const float *bias, int cout, int ntaps, int n_img, float *out,
                 cudaStream_t st)
 {
-    if (x.C == 64 && cout == 1 && ntaps == 9) return launch_narrow<64, 1, 9, ACT_SIGMOID, 0>(x, src_img, w, bias, n_img, out, 0, 0, 0, 0, st);
-    if (x.C == 64 && cout == 2 && ntaps == 1) return launch_narrow<64, 2, 1, ACT_SIGMOID, 0>(x, src_img, w, bias, n_img, out, 0, 0, 0, 0, st);
-    if (x.C == 32 && cout == 1 && ntaps == 9) return launch_narrow<32, 1, 9, ACT_SIGMOID, 0>(x, src_img, w, bias, n_img, out, 0, 0, 0, 0, st);
-    if (x.C == 16 && cout == 1 && ntaps == 9) return launch_narrow<16, 1, 9, ACT_SIGMOID, 0>(x, src_img, w, bias, n_img, out, 0, 0, 0, 0, st);
+    if (x.C == 64 && cout == 2 && ntaps == 1) return launch_narrow<64, 2, 1>(x, src_img, w, bias, n_img, out, st);
     set_error("conv_narrow: C=%d cout=%d taps=%d has no instantiation", x.C, cout, ntaps);
     return ESR_EINVAL;
-}
-
-// tail (models/model.py:337): 8 -> 2, 3x3, ReLU, fp32 NCHW output cropped back to the un-padded size (CropSize)
-int conv_narrow_tail(const SplitTensor &x, const float *w, const float *bias, int n_img, float *out, int crop_top, int crop_left, int out_H,
-                     int out_W, cudaStream_t st)
-{
-    ESR_REQUIRE(x.C == 8, "conv_narrow_tail: C=%d", x.C);
-    return launch_narrow<8, 2, 9, ACT_RELU, 1>(x, nullptr, w, bias, n_img, out, crop_top, crop_left, out_H, out_W, st);
 }
 
 // fp32 [Cout, 64, k, k] -> [tap][ci][co]

@@ -235,26 +235,6 @@ __global__ void __launch_bounds__(256) k_conv_mma(const DirectArgs a)
                 const __nv_bfloat16 *s = hi + (((size_t)simg * a.Hin + sy) * a.Win + sx) * CIN + q * 8;
                 float v[8];
                 dc_unpack8(__ldg(reinterpret_cast<const uint4 *>(s)), __ldg(reinterpret_cast<const uint4 *>(s + plane)), v);
-                if (a.agg_feats) {
-                    // scale aggregation fused into the fill (was a separate pass writing and re-reading a whole tensor):
-                    // x + (sum over the window's frames, in order, of feats * attention) * (1 / N), as k_scale_aggregate
-                    float acc[8];
-#pragma unroll
-                    for (int e = 0; e < 8; ++e) acc[e] = 0.0f;
-                    const size_t pix = (size_t)sy * a.Win + sx, HW = (size_t)a.Hin * a.Win;
-                    for (int n = 0; n < a.agg_N; ++n) {
-                        const size_t fp = (size_t)(a.agg_idx ? a.agg_idx[img * a.agg_N + n] : img * a.agg_N + n) * HW + pix;
-                        const __nv_bfloat16 *f = a.agg_feats + fp * CIN + q * 8;
-                        float fv[8];
-                        dc_unpack8(__ldg(reinterpret_cast<const uint4 *>(f)), __ldg(reinterpret_cast<const uint4 *>(f + a.agg_plane)), fv);
-                        const float at = __ldg(a.agg_att + fp);
-#pragma unroll
-                        for (int e = 0; e < 8; ++e) acc[e] += fv[e] * at;
-                    }
-                    const float inv = 1.0f / (float)a.agg_N;
-#pragma unroll
-                    for (int e = 0; e < 8; ++e) v[e] += acc[e] * inv;
-                }
                 float4 *d = reinterpret_cast<float4 *>(srcp + (size_t)sp * SPITCH + q * 32);
                 d[0] = make_float4(v[0], v[1], v[2], v[3]);
                 d[1] = make_float4(v[4], v[5], v[6], v[7]);

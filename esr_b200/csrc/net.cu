@@ -61,7 +61,7 @@ struct ParamLayout {
     size_t dw[D_COUNT], db[D_COUNT];     // direct layers
     size_t dm[D_COUNT];                  // the same weights as the split-bf16 image of the mma.sync kernels
     size_t fc0w, fc0b, fc1w, fc1b;
-    size_t nw_pm1, nw_at0, nw_ker;       // fp32 [tap][ci][co] weights of the narrow-output layers (conv_narrow)
+    size_t nw_ker;                       // fp32 [ci][co] weights of the spatial-attention kernel (conv_narrow)
     size_t total;
 };
 // Only dense_fusion.0's packed weight depends on N; the entries after it move with its size.  N = 3 is the layout of
@@ -83,7 +83,7 @@ static ParamLayout param_layout(int N)
         }
         l.fc0w = take(sizeof(float) * 32 * 64); l.fc0b = take(sizeof(float) * 32);
         l.fc1w = take(sizeof(float) * 128 * 32); l.fc1b = take(sizeof(float) * 128);
-        l.nw_pm1 = take(sizeof(float) * 9 * 64); l.nw_at0 = take(sizeof(float) * 9 * 64); l.nw_ker = take(sizeof(float) * 64 * 2);
+        l.nw_ker = take(sizeof(float) * 64 * 2);
         l.total = off;
     }
     return l;
@@ -112,10 +112,8 @@ struct Net {
     ConvTCArgs c_pm0, c_pm1, c_lf1, c_lf2, c_lf3, c_gx, c_gf, c_of0, c_of1, c_com, c_dcn, c_cb0, c_cb1, c_ker, c_df0, c_df1,
         c_dn0, c_dn1, c_at0, c_rc0;
     std::vector<ConvTCArgs> c_gzr, c_go;
-    void *gru_plan = nullptr;          // the ConvGRU recurrence as one cooperative launch (opt-in); nullptr = two launches per step
     void *dcn_plan = nullptr;          // fused sampling + contraction (dcn_fused.cu); nullptr = columns + 1x1 GEMM
     DirectArgs d[D_COUNT];
-    bool agg_fused = false;            // scale aggregation of decoder levels 1, 2 inside the recons convs' fill
 };
 
 static size_t split_bytes(int n_img, int H, int W, int C) { return (size_t)2 * n_img * H * W * C * sizeof(__nv_bfloat16); }
@@ -301,10 +299,6 @@ static int build(Net &n, cudaStream_t st)
         d.epi_mode = EPI_GRU_OUT; d.h_prev = view_imgs(n.hs, g * 2 * B); d.z_buf = n.zbuf; d.out = view_imgs(n.hs, (g + 1) * 2 * B);
         if ((rc = conv_tc_prepare(d, &n.c_go[g]))) return rc;
     }
-    // ESR_GRU_CHAIN=1: the whole chain as ONE cooperative kernel (bit-identical).  Opt-in: on H100 it measured no faster than two
-    // launches per step (cfg2: 6.61 / 6.68 vs 6.58 / 6.43 ms per step, alternating, DESIGN.md 8c) -- one 168-register CTA per SM and
-    // 36 grid barriers against PDL-overlapped launches with two CTAs per SM on the N = 64 phase.  Read per net, so a test can build both.
-    if (getenv("ESR_GRU_CHAIN") != nullptr && (rc = gru_chain_prepare(n.c_gzr, n.c_go, &n.gru_plan))) return rc;
     d = mk(n, T_GF, VN, ACT_RELU); d.n_src = 2; d.src[0] = n.hs; d.src_img[0] = n.m_gf_f; d.src[1] = n.hs; d.src_img[1] = n.m_gf_r;
     d.res_mode = RES_POST_ACT; d.res = n.F; d.res_img = n.m_gfres; d.out = n.tp;
     if ((rc = conv_tc_prepare(d, &n.c_gf))) return rc;
@@ -370,16 +364,8 @@ static int build(Net &n, cudaStream_t st)
     a = base(D_AT1, ACT_SIGMOID); in_split(a, n.t_e1); a.out_f32 = n.att1; a.Hout = n.t_e1.H; a.Wout = n.t_e1.W; a.n_img = FR; n.d[D_AT1] = a;
     a = base(D_AT2, ACT_SIGMOID); in_split(a, n.t_e0); a.out_f32 = n.att2; a.Hout = n.t_e0.H; a.Wout = n.t_e0.W; a.n_img = FR; n.d[D_AT2] = a;
     a = base(D_RC0, ACT_RELU); in_split(a, n.pre0); out_split(a, n.x1, VB); n.d[D_RC0] = a;
-    // scale aggregation (model.py:259-267) of the two full-resolution decoder levels CAN be folded into the fill of the recons convs
-    // (mma_conv.cu, DirectArgs::agg_*; ESR_AGG_FUSE=1): measured a net loss -- the two k_scale_aggregate launches (64 us) go away but the
-    // latency-bound fills grow by 37 + 38 us (profiles/r2_notes.md) -- so the separate bandwidth-bound pass stays the default.
-    n.agg_fused = getenv("ESR_AGG_FUSE") != nullptr && getenv("ESR_DIRECT_FFMA") == nullptr;
-    a = base(D_RC1, ACT_RELU); in_split(a, n.agg_fused ? n.x1 : n.pre1); out_split(a, n.x2, VB);
-    if (n.agg_fused) { a.agg_feats = n.t_e1.base; a.agg_plane = n.t_e1.plane(); a.agg_att = n.att1; a.agg_idx = n.m_fr; a.agg_N = N; }
-    n.d[D_RC1] = a;
-    a = base(D_RC2, ACT_RELU); in_split(a, n.agg_fused ? n.x2 : n.pre2); out_split(a, n.x3, VB);
-    if (n.agg_fused) { a.agg_feats = n.t_e0.base; a.agg_plane = n.t_e0.plane(); a.agg_att = n.att2; a.agg_idx = n.m_fr; a.agg_N = N; }
-    n.d[D_RC2] = a;
+    a = base(D_RC1, ACT_RELU); in_split(a, n.pre1); out_split(a, n.x2, VB); n.d[D_RC1] = a;
+    a = base(D_RC2, ACT_RELU); in_split(a, n.pre2); out_split(a, n.x3, VB); n.d[D_RC2] = a;
     a = base(D_TAIL, ACT_RELU); in_split(a, n.x3); a.Hout = n.Hc; a.Wout = n.Wc; a.n_img = VB;
     a.crop_top = n.pad_top; a.crop_left = n.pad_left; a.out_H = n.H; a.out_W = n.W; n.d[D_TAIL] = a;
     return ESR_OK;
@@ -429,12 +415,6 @@ static int forward(Net &n, const float *input, const int *in_img, float *output,
 #define RUND(name_, kind, dl, args) RUNC(name_, PC_DIRECT, direct_flops(dl, args), direct_bytes(dl, args), conv_direct(kind, args, st))
     const int B = n.B, N = n.N, VB = n.VB, VN = VB * N, nf = (N - 1) * VB, nsteps = n.Wn * N;
     const ParamLayout &L = n.P;
-    // Cout <= 2 layers on CUDA cores (elementwise.cu conv_narrow).  Measured (profiles/r2_notes.md): only the 1x1 spatial-attention
-    // kernel wins (18.8 -> 14.8 us); the 3x3 ones are latency-bound there (pred_map[1] 41 -> 51, tail 66 -> 93 us) and stay on the
-    // tensor-core / mma.sync kernels.  ESR_NARROW_ALL=1 routes all of them through conv_narrow, ESR_NARROW_TC=1 none.
-    static const bool narrow_all = getenv("ESR_NARROW_ALL") != nullptr;
-    static const bool narrow_ker = narrow_all || getenv("ESR_NARROW_TC") == nullptr;
-    const bool narrow = narrow_all;
     // ---- per-frame work, once per bank frame: head + encoder (models/model.py:329-331) and the three attention maps
     //      of scale_aggre (model.py:259-262), which depend on the encoder features only
     const double px = (double)n.h * n.w;             // feature-resolution pixels per image
@@ -443,21 +423,12 @@ static int forward(Net &n, const float *input, const int *in_img, float *output,
          4.0 * a.n_img * ((double)n.H * n.W * 2.0 + (double)a.Hout * a.Wout * 16.0), conv_direct(DK_HEAD_ENC0, a, st));
     RUND("enc1", DK_ENC1, D_ENC1, n.d[D_ENC1]);
     RUND("enc2", DK_ENC2, D_ENC2, n.d[D_ENC2]);
-    if (narrow) RUNC("atten0", PC_OTHER, 0.0, tc_bytes(n.c_at0), conv_narrow(n.F, nullptr, (const float *)(n.params + L.nw_at0), pb(n, T_AT0), 1, 9, n.FR, n.att0, st));
-    else RUNT("atten0", n.c_at0);
-    if (narrow) {
-        RUNC("atten1", PC_DIRECT, direct_flops(D_AT1, n.d[D_AT1]), direct_bytes(D_AT1, n.d[D_AT1]),
-             conv_narrow(n.t_e1, nullptr, n.d[D_AT1].w, n.d[D_AT1].bias, 1, 9, n.FR, n.att1, st));
-        RUNC("atten2", PC_DIRECT, direct_flops(D_AT2, n.d[D_AT2]), direct_bytes(D_AT2, n.d[D_AT2]),
-             conv_narrow(n.t_e0, nullptr, n.d[D_AT2].w, n.d[D_AT2].bias, 1, 9, n.FR, n.att2, st));
-    } else {
-        RUND("atten1", DK_ATT32, D_AT1, n.d[D_AT1]);
-        RUND("atten2", DK_ATT16, D_AT2, n.d[D_AT2]);
-    }
+    RUNT("atten0", n.c_at0);
+    RUND("atten1", DK_ATT32, D_AT1, n.d[D_AT1]);
+    RUND("atten2", DK_ATT16, D_AT2, n.d[D_AT2]);
     // ---- TimePropagation.local_time_corre for every window (model.py:77-89,133-146)
     RUNT("pred_map0", n.c_pm0);
-    if (narrow) RUNC("pred_map1", PC_OTHER, 0.0, tc_bytes(n.c_pm1), conv_narrow(n.t_pm0, nullptr, (const float *)(n.params + L.nw_pm1), pb(n, T_PM1), 1, 9, VB * (N + 1), n.maps, st));
-    else RUNT("pred_map1", n.c_pm1);
+    RUNT("pred_map1", n.c_pm1);
     RUN("ltc_cat", 4.0 * VN * px * (192.0 + 192.0 + 2.0), ltc_cat(n.F, n.maps, n.m_ltc5, VN, n.t_cat, st));
     RUNT("local_fusion.res.conv1", n.c_lf1);
     RUNT("local_fusion.res.conv2", n.c_lf2);
@@ -465,15 +436,9 @@ static int forward(Net &n, const float *input, const int *in_img, float *output,
     // ---- TimePropagation.global_time_corre: bidirectional ConvGRU (model.py:91-124); the only serial part:
     //      window after window, step after step, both directions batched as 2B images
     RUNT("gru.xconv", n.c_gx);
-    if (n.gru_plan) {
-        double fl = 0.0, by = 0.0;
-        for (int g = 0; g < nsteps; ++g) { fl += tc_flops(n.c_gzr[g]) + tc_flops(n.c_go[g]); by += tc_bytes(n.c_gzr[g]) + tc_bytes(n.c_go[g]); }
-        RUNC("gru.chain", PC_TC, fl, by, gru_chain_launch(n.gru_plan, st));
-    } else {
-        for (int g = 0; g < nsteps; ++g) {
-            RUNT("gru.zr", n.c_gzr[g]);
-            RUNT("gru.out", n.c_go[g]);
-        }
+    for (int g = 0; g < nsteps; ++g) {
+        RUNT("gru.zr", n.c_gzr[g]);
+        RUNT("gru.out", n.c_go[g]);
     }
     RUNT("global_fusion", n.c_gf);
     // carried states: the last slot becomes slot 0 of the next call
@@ -490,8 +455,7 @@ static int forward(Net &n, const float *input, const int *in_img, float *output,
     }
     RUNT("convblock0", n.c_cb0);
     RUNT("convblock1", n.c_cb1);
-    if (narrow_ker) RUNC("spatial_kernel", PC_OTHER, 0.0, tc_bytes(n.c_ker), conv_narrow(n.feat, nullptr, (const float *)(n.params + L.nw_ker), pb(n, T_KER), 2, 1, nf, n.sk, st));
-    else RUNT("spatial_kernel", n.c_ker);
+    RUNC("spatial_kernel", PC_OTHER, 0.0, tc_bytes(n.c_ker), conv_narrow(n.feat, nullptr, (const float *)(n.params + L.nw_ker), pb(n, T_KER), 2, 1, nf, n.sk, st));
     RUN("chan_max", 4.0 * nf * px * 64.0, chan_max(n.feat, nf, n.mx, st));
     RUN("attn_mlp", 4.0 * nf * 192.0, attn_mlp(n.mx, nf, (const float *)(n.params + L.fc0w), (const float *)(n.params + L.fc0b),
                  (const float *)(n.params + L.fc1w), (const float *)(n.params + L.fc1b), n.ck, st));
@@ -505,13 +469,13 @@ static int forward(Net &n, const float *input, const int *in_img, float *output,
     RUN("scale_aggre0", 4.0 * VB * px * (64.0 * (2 + N) + N), scale_aggregate(n.x0, n.F, n.att0, n.m_fr, VB, N, n.pre0, st));
     RUN("upsample2x", 4.0 * VB * px * 64.0 * 5.0, upsample2x(n.pre0, VB, n.up0, st));
     RUNT("recons0", n.c_rc0);
-    if (!n.agg_fused) RUN("scale_aggre1", 4.0 * VB * 4.0 * px * (32.0 * (2 + N) + N), scale_aggregate(n.x1, n.t_e1, n.att1, n.m_fr, VB, N, n.pre1, st));
+    RUN("scale_aggre1", 4.0 * VB * 4.0 * px * (32.0 * (2 + N) + N), scale_aggregate(n.x1, n.t_e1, n.att1, n.m_fr, VB, N, n.pre1, st));
     RUND("recons1", DK_RECON1, D_RC1, n.d[D_RC1]);
-    if (!n.agg_fused) RUN("scale_aggre2", 4.0 * VB * 16.0 * px * (16.0 * (2 + N) + N), scale_aggregate(n.x2, n.t_e0, n.att2, n.m_fr, VB, N, n.pre2, st));
+    RUN("scale_aggre2", 4.0 * VB * 16.0 * px * (16.0 * (2 + N) + N), scale_aggregate(n.x2, n.t_e0, n.att2, n.m_fr, VB, N, n.pre2, st));
     RUND("recons2", DK_RECON2, D_RC2, n.d[D_RC2]);
     a = n.d[D_TAIL]; a.out_f32 = output;
     RUNC("tail", PC_DIRECT, direct_flops(D_TAIL, a), 4.0 * a.n_img * ((double)n.Hc * n.Wc * 8.0 + (double)n.H * n.W * 2.0),
-         narrow ? conv_narrow_tail(n.x3, a.w, a.bias, VB, output, n.pad_top, n.pad_left, n.H, n.W, st) : conv_direct(DK_TAIL, a, st));
+         conv_direct(DK_TAIL, a, st));
 #undef RUN
 #undef RUNT
 #undef RUND
@@ -567,8 +531,6 @@ extern "C" int esr_net_pack_params_n(int num_frame, const float *const *p, void 
     ESR_CUDA_CHECK(cudaMemcpyAsync(out + L.fc0b, p[P_FC0_B], sizeof(float) * 32, cudaMemcpyDeviceToDevice, st));
     ESR_CUDA_CHECK(cudaMemcpyAsync(out + L.fc1w, p[P_FC1_W], sizeof(float) * 128 * 32, cudaMemcpyDeviceToDevice, st));
     ESR_CUDA_CHECK(cudaMemcpyAsync(out + L.fc1b, p[P_FC1_B], sizeof(float) * 128, cudaMemcpyDeviceToDevice, st));
-    if ((rc = pack_narrow_weight(p[P_PM1_W], 1, 9, (float *)(out + L.nw_pm1), st))) return rc;
-    if ((rc = pack_narrow_weight(p[P_AT0_W], 1, 9, (float *)(out + L.nw_at0), st))) return rc;
     if ((rc = pack_narrow_weight(p[P_KER_W], 2, 1, (float *)(out + L.nw_ker), st))) return rc;
     return ESR_OK;
 }
@@ -631,7 +593,6 @@ extern "C" int esr_net_create(esr_net_t *out, int B, int N, int L, int H, int W,
 extern "C" int esr_net_destroy(esr_net_t net)
 {
     if (net && ((Net *)net)->dcn_plan) dcn_fused_destroy(((Net *)net)->dcn_plan);
-    if (net && ((Net *)net)->gru_plan) gru_chain_destroy(((Net *)net)->gru_plan);
     delete (Net *)net;
     return ESR_OK;
 }

@@ -28,9 +28,6 @@ struct DirectArgs {
     size_t out_plane = 0;
     float *out_f32 = nullptr;
     int crop_top = 0, crop_left = 0, out_H = 0, out_W = 0;          // NCHW output window (tail)
-    // decoder layers (bilinear x2 fused): optional scale aggregation folded into the source-patch fill (models/model.py:259-267):
-    //   source value = in_split[b] + mean_n(agg_feats[agg_idx[b * agg_N + n]] * agg_att[same pixel])
-    const __nv_bfloat16 *agg_feats = nullptr; size_t agg_plane = 0; const float *agg_att = nullptr; const int *agg_idx = nullptr; int agg_N = 0;
 };
 
 int conv_direct(DirectKind kind, const DirectArgs &a, cudaStream_t st);
@@ -68,8 +65,6 @@ int copy_split(const SplitTensor &src, const int *src_img, int n_img, const Spli
 int conv_narrow(const SplitTensor &x, const int *src_img, const float *w, const float *bias, int cout, int ntaps, int n_img, float *out,
                 cudaStream_t st);
 int pack_narrow_weight(const float *w, int cout, int ntaps, float *dst, cudaStream_t st);
-int conv_narrow_tail(const SplitTensor &x, const float *w, const float *bias, int n_img, float *out, int crop_top, int crop_left, int out_H,
-                     int out_W, cudaStream_t st);
 
 // ---- deformable sampling (dcn.cu): columns[img][y][x][tap*64 + c] = bilinear(feat[c], y-1+i+off_h, x-1+j+off_w) * mask
 // om: fp32 NHWC [n_img, H, W, 216] = {144 offsets (group-major, (h,w) pairs per tap), 72 masks (already sigmoid)}

@@ -34,7 +34,7 @@ constexpr int TC_THREADS = 288;
 // rows into it (a multiple of 1024 bytes, so every tap starts on a SWIZZLE_128B atom).  A 1x1 layer loads the tile itself, one
 // tap per box.  A boxes and per-tap weights (B) have separate rings: a consumer frees an A box once the MMAs of its last tap
 // retired, and each B slot once its own MMAs did.  The TMA producer streams both across tile boundaries, so the loads of
-// tile i+1 overlap the epilogue of tile i; the ring positions of each role persist across tiles and calls.
+// tile i+1 overlap the epilogue of tile i; the ring positions of each role persist across tiles.
 // The epilogue stages accumulators in a dedicated area beside the rings (the rings are already refilling).
 // ------------------------------------------------------------------------------------------------
 struct TcSmem {
@@ -48,14 +48,13 @@ struct TcSmem {
     __device__ uint32_t b_empty(uint32_t s) const { return bar + 8u * (2 * na + nb + s); }
 };
 // Ring position: the count of slots used modulo twice the depth n, i.e. slot c % n with phase c / n (one register per ring).
-struct TcRing { uint32_t ca = 0, cb = 0; };
 __device__ __forceinline__ uint32_t ring_slot(uint32_t c, int n) { return c < (uint32_t)n ? c : c - n; }
 __device__ __forceinline__ uint32_t ring_phase(uint32_t c, int n) { return c < (uint32_t)n ? 0u : 1u; }
 __device__ __forceinline__ uint32_t ring_next(uint32_t c, int n) { return c + 1 == 2u * n ? 0u : c + 1; }
 __device__ __forceinline__ uint32_t ring_prev_slot(uint32_t c, int n) { return ring_slot(c == 0 ? 2u * n - 1 : c - 1, n); }
 
 // 1024: worst-case alignment of the rings; then the A ring, the B ring, the two staging tiles and the full / empty mbarriers of
-// both rings.  conv_tc_prepare and gru_chain_prepare size the rings so that this fits the 227 KB (232448 B) an H100 block
+// both rings.  conv_tc_prepare sizes the rings so that this fits the 227 KB (232448 B) an H100 block
 // may opt in to.
 static size_t tc_smem_bytes(int npad, uint32_t a_box, int na, int nb)
 {
@@ -109,7 +108,7 @@ __device__ __forceinline__ void tc_init_barriers(const TcSmem &m)
 // KS = 0: 3x3 or 1x1 (a.ntaps 9 or 1); KS = 5: 5x5, pad 2 (a.ntaps 25) -- one box of TW x (TH + 4) pixels per (chunk, dx),
 // read by the five dy taps, and the packing's order chunk * 25 + 5 (dy + 2) + dx + 2.
 template <int NP, int KS = 0>
-__device__ __forceinline__ void conv_tiles(const ConvTCArgs &a, int tile0, int step, const TcSmem &m, TcRing &ring)
+__device__ __forceinline__ void conv_tiles(const ConvTCArgs &a, int tile0, int step, const TcSmem &m)
 {
     static_assert(KS == 0 || KS == 5, "conv_tiles: KS is 0 (3x3 / 1x1) or 5");
     constexpr bool k5 = KS == 5;
@@ -123,7 +122,7 @@ __device__ __forceinline__ void conv_tiles(const ConvTCArgs &a, int tile0, int s
     if (warp == 8) {
         // ===================== TMA producer (one elected lane; the others idle until the caller's next barrier) =====================
         if (elect_one_sync()) {
-            uint32_t ca = ring.ca, cb = ring.cb;
+            uint32_t ca = 0, cb = 0;
             for (int tile = tile0; tile < n_tiles; tile += step) {
                 const int img = tile / tiles_per_img, trem = tile - img * tiles_per_img;
                 const int y0 = (trem / a.tiles_x) * a.TH, x0 = (trem % a.tiles_x) * a.TW;
@@ -155,7 +154,6 @@ __device__ __forceinline__ void conv_tiles(const ConvTCArgs &a, int tile0, int s
                     }
                 }
             }
-            ring.ca = ca; ring.cb = cb;
         }
         return;
     }
@@ -165,7 +163,7 @@ __device__ __forceinline__ void conv_tiles(const ConvTCArgs &a, int tile0, int s
     float *stg = m.stg + wg * (TC_STG_BYTES / 4);
     const int r = threadIdx.x & 63, h = (threadIdx.x >> 6) & 1;
     const uint32_t tap_rows = (uint32_t)a.TW * 128u;                   // bytes between the dy taps of a box
-    uint32_t ca = ring.ca, cb = ring.cb;
+    uint32_t ca = 0, cb = 0;
     for (int tile = tile0; tile < n_tiles; tile += step) {
         const int img = tile / tiles_per_img, trem = tile - img * tiles_per_img;
         const int y0 = (trem / a.tiles_x) * a.TH, x0 = (trem % a.tiles_x) * a.TW;
@@ -228,7 +226,6 @@ __device__ __forceinline__ void conv_tiles(const ConvTCArgs &a, int tile0, int s
             named_sync(2 + wg, 128);
         }
     }
-    ring.ca = ca; ring.cb = cb;
 }
 
 // one layer: grid = min(tiles, resident CTAs); CTA b takes tiles b, b + gridDim.x, ...
@@ -240,44 +237,7 @@ __global__ void __launch_bounds__(TC_THREADS, 1) k_conv_tc(const __grid_constant
     const TcSmem m = tc_smem_layout(NP, a_box, a.a_stages, a.b_stages);
     tc_init_barriers(m);
     PDL_WAIT();                      // everything above is CTA-local set-up; global memory only from here on
-    TcRing ring;
-    conv_tiles<NP, KS>(a, blockIdx.x, gridDim.x, m, ring);
-}
-
-// ------------------------------------------------------------------------------------------------
-// The whole ConvGRU recurrence of a sequence batch in ONE cooperative launch: phases 2g (update|reset gates, N = 128, epilogue
-// z -> z_buf, h*r -> rh) and 2g + 1 (candidate, N = 64, epilogue h' = h (1 - z) + tanh(.) z) of step g, each a persistent pass
-// over the step's tiles, separated by a grid barrier.  The next phase's TMA loads read what other CTAs stored with ordinary
-// stores, so every thread fences its stores into the async proxy before the barrier and after it.
-// ------------------------------------------------------------------------------------------------
-__device__ __forceinline__ void grid_barrier(unsigned int *ctr, unsigned int target)
-{
-    asm volatile("fence.proxy.async.global;" ::: "memory");
-    __syncthreads();
-    if (threadIdx.x == 0) {
-        __threadfence();
-        atomicAdd(ctr, 1u);
-        unsigned int v;
-        do {
-            asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(ctr) : "memory");
-            if (v < target) __nanosleep(32);
-        } while (v < target);
-    }
-    __syncthreads();
-    asm volatile("fence.proxy.async.global;" ::: "memory");
-}
-
-__global__ void __launch_bounds__(TC_THREADS, 1) k_gru_chain(const ConvTCArgs *__restrict__ args, int nphase, int na, int nb,
-                                                             unsigned int *ctr)
-{
-    const TcSmem m = tc_smem_layout(128, tc_a_box_bytes(args[0].TW, args[0].TH, args[0].ntaps), na, nb);
-    tc_init_barriers(m);
-    TcRing ring;
-    for (int p = 0; p < nphase; ++p) {
-        if (p & 1) conv_tiles<64>(args[p], blockIdx.x, gridDim.x, m, ring);
-        else conv_tiles<128>(args[p], blockIdx.x, gridDim.x, m, ring);
-        grid_barrier(ctr, (unsigned int)(p + 1) * gridDim.x);
-    }
+    conv_tiles<NP, KS>(a, blockIdx.x, gridDim.x, m);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -444,68 +404,6 @@ int conv_tc_launch(const ConvTCArgs &a, cudaStream_t st)
     }
     set_error("conv_tc: npad=%d", a.npad);
     return ESR_EINVAL;
-}
-
-struct GruChainPlan { ConvTCArgs *args = nullptr; unsigned int *ctr = nullptr; int nphase = 0, na = 2, nb = 2; unsigned grid = 0; size_t smem = 0; };
-
-int gru_chain_prepare(const std::vector<ConvTCArgs> &zr, const std::vector<ConvTCArgs> &go, void **plan_out)
-{
-    ESR_REQUIRE(!zr.empty() && zr.size() == go.size(), "gru_chain: %zu / %zu steps", zr.size(), go.size());
-    GruChainPlan *p = new GruChainPlan();
-    std::vector<ConvTCArgs> ph;
-    for (size_t g = 0; g < zr.size(); ++g) {
-        if (zr[g].npad != 128 || go[g].npad != 64 || zr[g].epi_mode != EPI_GRU_ZR || go[g].epi_mode != EPI_GRU_OUT) {
-            delete p; set_error("gru_chain: unexpected gate layers"); return ESR_EINVAL;
-        }
-        ph.push_back(zr[g]); ph.push_back(go[g]);
-    }
-    p->nphase = (int)ph.size();
-    // both phases share one layout: A boxes of the (common) tile shape, B slots of the wider (128) phase
-    const size_t cap = (size_t)dev_info().max_smem_optin;
-    const uint32_t a_box = tc_a_box_bytes(zr[0].TW, zr[0].TH, zr[0].ntaps);
-    if (!tc_rings(128, a_box, zr[0].ntaps == 9 ? 3 : 1, cap, &p->na, &p->nb)) {
-        delete p; set_error("gru_chain: the rings do not fit in shared memory"); return ESR_EINVAL;
-    }
-    p->smem = tc_smem_bytes(128, a_box, p->na, p->nb);
-    cudaError_t e = cudaFuncSetAttribute(k_gru_chain, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)p->smem);
-    int per_sm = 0;
-    if (e == cudaSuccess) e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_gru_chain, TC_THREADS, p->smem);
-    if (e == cudaSuccess && per_sm < 1) e = cudaErrorInvalidConfiguration;
-    const int n_tiles = zr[0].n_img * zr[0].tiles_x * zr[0].tiles_y;
-    p->grid = (unsigned)std::min(n_tiles, per_sm * dev_info().sm_count);      // all CTAs co-resident (cooperative launch)
-    if (e == cudaSuccess) e = cudaMalloc(&p->args, sizeof(ConvTCArgs) * ph.size());
-    if (e == cudaSuccess) e = cudaMalloc(&p->ctr, 256);
-    if (e == cudaSuccess) e = cudaMemcpy(p->args, ph.data(), sizeof(ConvTCArgs) * ph.size(), cudaMemcpyHostToDevice);
-    if (e != cudaSuccess) {
-        set_error("gru_chain: %s", cudaGetErrorString(e));
-        cudaFree(p->args); cudaFree(p->ctr); delete p;
-        return ESR_ECUDA;
-    }
-    *plan_out = p;
-    return ESR_OK;
-}
-
-int gru_chain_launch(void *plan, cudaStream_t st)
-{
-    GruChainPlan *p = (GruChainPlan *)plan;
-    ESR_CUDA_CHECK(cudaMemsetAsync(p->ctr, 0, sizeof(unsigned int), st));
-    cudaLaunchConfig_t cfg{};
-    cfg.gridDim = dim3(p->grid); cfg.blockDim = dim3(TC_THREADS); cfg.dynamicSmemBytes = p->smem; cfg.stream = st;
-    cudaLaunchAttribute at[1];
-    at[0].id = cudaLaunchAttributeCooperative;
-    at[0].val.cooperative = 1;
-    cfg.attrs = at; cfg.numAttrs = 1;
-    ESR_CUDA_CHECK(cudaLaunchKernelEx(&cfg, k_gru_chain, (const ConvTCArgs *)p->args, p->nphase, p->na, p->nb, p->ctr));
-    esr::count_launch();
-    return ESR_OK;
-}
-
-void gru_chain_destroy(void *plan)
-{
-    GruChainPlan *p = (GruChainPlan *)plan;
-    if (!p) return;
-    cudaFree(p->args); cudaFree(p->ctr);
-    delete p;
 }
 
 // ------------------------------------------------------------------------------------------------

@@ -2,7 +2,6 @@
 #pragma once
 #include "common.cuh"
 #include <cuda.h>   // CUtensorMap (types only; the driver entry point is resolved at run time)
-#include <vector>
 
 namespace esr {
 enum Act : int { ACT_NONE = 0, ACT_RELU = 1, ACT_SIGMOID = 2, ACT_TANH = 3 };
@@ -88,10 +87,6 @@ static inline size_t tc_packed_weight_bytes(int cout, int cin_total, int ntaps)
 // Builds tensor maps + launch geometry.  H, W taken from src[0].
 int conv_tc_prepare(const ConvTCDesc &d, ConvTCArgs *args);
 int conv_tc_launch(const ConvTCArgs &args, cudaStream_t st);
-// the ConvGRU recurrence as one cooperative launch over the prepared gate layers of every step (EPI_GRU_ZR / EPI_GRU_OUT)
-int gru_chain_prepare(const std::vector<ConvTCArgs> &zr, const std::vector<ConvTCArgs> &go, void **plan_out);
-int gru_chain_launch(void *plan, cudaStream_t st);
-void gru_chain_destroy(void *plan);
 // tensor-map builders (shared with dcn_fused.cu, wgrad_tc.cu)
 int tc_make_amap(const SplitTensor &t, int box_w, int box_h, CUtensorMap *out);
 int tc_make_bmap(const void *w, int npad, int nkb, int box_rows, CUtensorMap *out);

@@ -598,122 +598,6 @@ __global__ void __launch_bounds__(256) k_conv_wgrad_g_det(const float *__restric
 }
 
 // ------------------------------------------------------------------------------------------------------------------
-// dw of the narrow 3x3 layers on the warp-level tensor cores.  Per tap the weight gradient is a GEMM over pixels:
-//   D[co][n] += sum_px g[co][px] * x[ci(n)][py(px) * s + ky(n)][px(px) * s + kx(n)],   n = ci * 9 + tap  (= the dw memory order)
-// mma.sync m16n8k16 with A = g (row-major, K = 16 consecutive output pixels of a tile row) and B = shifted x (col-major: two
-// consecutive pixels per register).  fp32 inputs are split to bf16 (hi, lo) while staging a 16x16 output tile in shared
-// memory -- g as [co][pixel], x as three column-shifted copies (one per kx) of PACKED pixel pairs so that every B fragment is
-// one aligned 32-bit load for both strides -- and the usual three products (lo*hi + hi*lo + hi*hi) accumulate in fp32.
-// Block = (16 output channels, 8 input channels) x a slice of the (image, tile) items; warp w owns tile rows w and w + 8;
-// partial sums are combined through shared-memory atomics and added to dw once per block.
-// ------------------------------------------------------------------------------------------------------------------
-constexpr int WM_GP = 264;                                         // g row pitch (bf16 elements): conflict-free A fragment loads
-
-__device__ __forceinline__ uint32_t pack_bf16x2(__nv_bfloat16 a, __nv_bfloat16 b)
-{
-    return (uint32_t)__bfloat16_as_ushort(a) | ((uint32_t)__bfloat16_as_ushort(b) << 16);
-}
-__device__ __forceinline__ void mma_bf16_k16(float (&d)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1)
-{
-    asm volatile("mma.sync.aligned.m16n8k16.row.col.f32.bf16.bf16.f32 {%0, %1, %2, %3}, {%4, %5, %6, %7}, {%8, %9}, {%0, %1, %2, %3};"
-                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]) : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
-}
-
-template <int STRIDE>
-__global__ void __launch_bounds__(256) k_conv_wgrad_mma(const float *__restrict__ x, const float *__restrict__ g, float *__restrict__ dw,
-                                                        int B, int Cin, int H, int W, int Cout, int Ho, int Wo)
-{
-    constexpr int PD = 15 * STRIDE + 3;                            // input rows needed by a 16-row output tile
-    constexpr int XW = 8 * PD * 8;                                 // words per (copy, plane): [ci 8][row PD][pair 8]
-    extern __shared__ __align__(16) uint8_t wsm_raw[];
-    __nv_bfloat16 *g_hi = reinterpret_cast<__nv_bfloat16 *>(wsm_raw), *g_lo = g_hi + 16 * WM_GP;
-    uint32_t *x_hi = reinterpret_cast<uint32_t *>(g_lo + 16 * WM_GP), *x_lo = x_hi + 3 * XW;
-    float *red = reinterpret_cast<float *>(x_lo + 3 * XW);          // [16][72] block-level partial sums
-
-    const int ci_tiles = (Cin + 7) / 8;
-    const int co0 = (blockIdx.x / ci_tiles) * 16, ci0 = (blockIdx.x % ci_tiles) * 8;
-    const int tiles_x = (Wo + 15) / 16, tiles_y = (Ho + 15) / 16;
-    const int items = B * tiles_x * tiles_y;
-    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, gq = lane >> 2, t4 = lane & 3;
-    float acc[9][4];
-#pragma unroll
-    for (int n = 0; n < 9; ++n) acc[n][0] = acc[n][1] = acc[n][2] = acc[n][3] = 0.0f;
-    for (int i = tid; i < 16 * 72; i += 256) red[i] = 0.0f;
-
-    for (int it = blockIdx.y; it < items; it += gridDim.y) {
-        const int n_img = it / (tiles_x * tiles_y), tr = it % (tiles_x * tiles_y);
-        const int ty0 = (tr / tiles_x) * 16, tx0 = (tr % tiles_x) * 16;
-        __syncthreads();                                            // previous item's fragments are consumed
-        // ---- stage g: 16 channels x 256 pixels, split
-        for (int i = tid; i < 16 * 256; i += 256) {
-            const int co = i >> 8, p = i & 255;
-            const int oy = ty0 + (p >> 4), ox = tx0 + (p & 15);
-            float v = 0.0f;
-            if (co0 + co < Cout && oy < Ho && ox < Wo) v = g[(((size_t)n_img * Cout + co0 + co) * Ho + oy) * Wo + ox];
-            __nv_bfloat16 h, l;
-            split_bf16(v, h, l);
-            g_hi[co * WM_GP + p] = h;
-            g_lo[co * WM_GP + p] = l;
-        }
-        // ---- stage x: for each kx the pixel pairs (ox = 2j, 2j + 1) -> input columns (2j * s + kx, (2j + 1) * s + kx), packed
-        for (int i = tid; i < 3 * XW; i += 256) {
-            const int j = i & 7, row = (i >> 3) % PD, ci = (i / (8 * PD)) & 7, kx = i / XW;
-            const int iy = ty0 * STRIDE - 1 + row;
-            const int ix0 = (tx0 + 2 * j) * STRIDE - 1 + kx, ix1 = ix0 + STRIDE;
-            float v0 = 0.0f, v1 = 0.0f;
-            if (ci0 + ci < Cin && iy >= 0 && iy < H) {
-                const float *xr = x + (((size_t)n_img * Cin + ci0 + ci) * H + iy) * W;
-                if (ix0 >= 0 && ix0 < W) v0 = __ldg(xr + ix0);
-                if (ix1 >= 0 && ix1 < W) v1 = __ldg(xr + ix1);
-            }
-            __nv_bfloat16 h0, l0, h1, l1;
-            split_bf16(v0, h0, l0);
-            split_bf16(v1, h1, l1);
-            x_hi[i] = pack_bf16x2(h0, h1);
-            x_lo[i] = pack_bf16x2(l0, l1);
-        }
-        __syncthreads();
-        // ---- two K steps per warp: tile rows warp and warp + 8
-#pragma unroll
-        for (int kk = 0; kk < 2; ++kk) {
-            const int oyl = warp + 8 * kk;                          // tile row = K step
-            uint32_t ah[4], al[4];
-            {
-                const int o0 = gq * WM_GP + oyl * 16 + 2 * t4, o1 = (gq + 8) * WM_GP + oyl * 16 + 2 * t4;
-                ah[0] = *reinterpret_cast<const uint32_t *>(g_hi + o0); ah[1] = *reinterpret_cast<const uint32_t *>(g_hi + o1);
-                ah[2] = *reinterpret_cast<const uint32_t *>(g_hi + o0 + 8); ah[3] = *reinterpret_cast<const uint32_t *>(g_hi + o1 + 8);
-                al[0] = *reinterpret_cast<const uint32_t *>(g_lo + o0); al[1] = *reinterpret_cast<const uint32_t *>(g_lo + o1);
-                al[2] = *reinterpret_cast<const uint32_t *>(g_lo + o0 + 8); al[3] = *reinterpret_cast<const uint32_t *>(g_lo + o1 + 8);
-            }
-#pragma unroll
-            for (int nt = 0; nt < 9; ++nt) {
-                const int n = nt * 8 + gq;                          // this lane's B column: (ci, tap)
-                const int ci = n / 9, tap = n - ci * 9, ky = tap / 3, kx = tap - ky * 3;
-                const int wofs = kx * XW + (ci * PD + oyl * STRIDE + ky) * 8 + t4;
-                const uint32_t bh0 = x_hi[wofs], bh1 = x_hi[wofs + 4], bl0 = x_lo[wofs], bl1 = x_lo[wofs + 4];
-                mma_bf16_k16(acc[nt], al, bh0, bh1);
-                mma_bf16_k16(acc[nt], ah, bl0, bl1);
-                mma_bf16_k16(acc[nt], ah, bh0, bh1);
-            }
-        }
-    }
-    // ---- combine the 8 warps, then one global atomic per (co, n)
-    __syncthreads();
-#pragma unroll
-    for (int nt = 0; nt < 9; ++nt) {
-        atomicAdd(&red[gq * 72 + nt * 8 + 2 * t4], acc[nt][0]);
-        atomicAdd(&red[gq * 72 + nt * 8 + 2 * t4 + 1], acc[nt][1]);
-        atomicAdd(&red[(gq + 8) * 72 + nt * 8 + 2 * t4], acc[nt][2]);
-        atomicAdd(&red[(gq + 8) * 72 + nt * 8 + 2 * t4 + 1], acc[nt][3]);
-    }
-    __syncthreads();
-    for (int i = tid; i < 16 * 72; i += 256) {
-        const int co = i / 72, n = i % 72, ci = n / 9, tap = n % 9;
-        if (co0 + co < Cout && ci0 + ci < Cin) atomicAdd(dw + ((size_t)(co0 + co) * Cin + ci0 + ci) * 9 + tap, red[i]);
-    }
-}
-
-// ------------------------------------------------------------------------------------------------------------------
 // bilinear x2 (F.interpolate(scale_factor=2, mode='bilinear', align_corners=False), models/submodules.py:290) on fp32 NCHW
 // planes, forward and backward.  For scale 2 the source coordinate is oy/2 - 0.25, so output row 2k reads rows (k-1, k)
 // with weights (0.25, 0.75) and row 2k+1 reads (k, k+1) with (0.75, 0.25), clamped at the borders; the backward is the
@@ -960,11 +844,6 @@ static int launch_generic(int which, const float *x, const float *w, const float
     constexpr int KK = KS * KS;
     const dim3 blk(G_T, G_T);
     if (which == 2 && part) {
-        if (KS == 3 && getenv("ESR_WGRAD_MMA") != nullptr) {
-            set_error("conv2d_backward: the ESR_WGRAD_MMA weight gradient sums with atomics and has no deterministic variant; "
-                      "unset ESR_WGRAD_MMA or leave deterministic mode");
-            return ESR_EUNSUPPORTED;
-        }
         const int PD = (G_T - 1) * stride + KS;
         const size_t smem = (size_t)(256 * G_C + G_C * PD * PD) * 4;
         const int pairs = ((Cout + G_C - 1) / G_C) * ((Cin + G_C - 1) / G_C);
@@ -984,24 +863,6 @@ static int launch_generic(int which, const float *x, const float *w, const float
         const size_t smem = (size_t)(G_C * R_PH * R_PW + G_C * 9 * G_C) * 4;
         const dim3 grid(((Wo + R_TW - 1) / R_TW) * ((Ho + R_TH - 1) / R_TH), (Cout + G_C - 1) / G_C, B);
         k_conv_fwd_r<<<grid, 256, smem, st>>>(x, w, bias, out, Cin, H, W, Cout, act);
-    } else if (which == 2 && KS == 3 && getenv("ESR_WGRAD_MMA") != nullptr) {
-        // opt-in experiment: parity-green but staging-bound (the three packed copies of the x patch cost more global loads than
-        // the FFMA kernel's single patch): 3.29 ms vs 3.35 ms for the narrow layers of a cfg2 iteration, +0.7 ms on the whole step
-        const int PD = 15 * stride + 3;
-        const size_t smem = (size_t)2 * 16 * WM_GP * 2 + (size_t)2 * 3 * 8 * PD * 8 * 4 + 16 * 72 * 4;
-        const int pairs = ((Cout + 15) / 16) * ((Cin + 7) / 8);
-        const int items = B * ((Wo + 15) / 16) * ((Ho + 15) / 16);
-        int slices = (dev_info().sm_count * 4 + pairs - 1) / pairs;
-        if (slices > items) slices = items;
-        if (slices < 1) slices = 1;
-        static bool attr = false;
-        if (!attr) {
-            ESR_CUDA_CHECK(cudaFuncSetAttribute(k_conv_wgrad_mma<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024));
-            ESR_CUDA_CHECK(cudaFuncSetAttribute(k_conv_wgrad_mma<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024));
-            attr = true;
-        }
-        if (stride == 1) k_conv_wgrad_mma<1><<<dim3(pairs, slices), 256, smem, st>>>(x, g, out, B, Cin, H, W, Cout, Ho, Wo);
-        else k_conv_wgrad_mma<2><<<dim3(pairs, slices), 256, smem, st>>>(x, g, out, B, Cin, H, W, Cout, Ho, Wo);
     } else if (which == 2 && KS == 3) {
         const int PD = (G_T - 1) * stride + 3;
         const size_t smem = (size_t)(256 * G_C + G_C * PD * PD) * 4;

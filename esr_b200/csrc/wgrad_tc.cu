@@ -197,13 +197,11 @@ __global__ void __launch_bounds__(WG_THREADS, 1) k_wgrad_tc(const __grid_constan
 __global__ void __launch_bounds__(WG_THREADS, 1) k_wgrad_tc_det(const __grid_constant__ WgradArgs a) { wgrad_tc_body<true>(a); }
 
 // CTAs per (M block, N chunk, tap group): one CTA per SM in all.  (Every CTA ends with 128 x 64 x taps fp32 atomics; giving small
-// problems fewer, longer CTAs was measured slower: min 6 tiles per CTA +0.3 ms, min 16 +2 ms per cfg2 training iteration --
-// ESR_WGRAD_MIN_TILES to retest.)
+// problems fewer, longer CTAs was measured slower: min 6 tiles per CTA +0.3 ms, min 16 +2 ms per cfg2 training iteration.)
 static int wgrad_tc_slices(int n_tiles, int base)
 {
     int slices = (dev_info().sm_count + base - 1) / base;
-    static const int min_tiles = getenv("ESR_WGRAD_MIN_TILES") ? atoi(getenv("ESR_WGRAD_MIN_TILES")) : 1;
-    if (slices > n_tiles / min_tiles) slices = n_tiles / min_tiles;
+    if (slices > n_tiles) slices = n_tiles;
     if (slices < 1) slices = 1;
     return slices;
 }

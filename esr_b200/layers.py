@@ -101,7 +101,7 @@ def conv_tc(srcs, wpacked, bias, cout, ntaps=9, act=None, act_from=0, src_img=No
 
 # esr_conv_small kinds (include/esr_b200.h) and paths
 SMALL_KINDS = {"head_enc0": 0, "enc1": 1, "enc2": 2, "att32": 3, "att16": 4, "recon1": 5, "recon2": 6, "tail": 7,
-               "pred_map1": 8, "atten0": 9, "spatial_kernel": 10}
+               "spatial_kernel": 10}
 SMALL_PATHS = {"mma": 0, "ffma": 1, "narrow": 2}
 
 
@@ -110,11 +110,10 @@ def conv_small_supported(kind, path):
 
 
 def conv_small(kind, path, x, w, bias, n_img, out=None, out_f32=None, in_img=None, pads=(0, 0, 0, 0), head=None,
-               crop=None, agg=None):
+               crop=None):
     """One small-channel / narrow-output layer of the network (esr_conv_small) on kernel family `path`.
     x: Split, or fp32 NCHW [*, 2, H, W] for head_enc0 (then head = (w_head, b_head), pads = (top, bottom, left, right));
-    out: Split for Cout >= 8, else out_f32 (NHWC, or NCHW [n_img, 2, out_H, out_W] with crop = (top, left) for the tail);
-    agg = (feats Split, att fp32 [feats.n_img, H, W], idx int [n_img * N] or None, N) for recon1 / recon2."""
+    out: Split for Cout >= 8, else out_f32 (NHWC, or NCHW [n_img, 2, out_H, out_W] with crop = (top, left) for the tail)."""
     L = _lib.lib()
     k, p = SMALL_KINDS[kind], SMALL_PATHS[path]
     d = _lib.ConvSmallDesc()
@@ -146,11 +145,6 @@ def conv_small(kind, path, x, w, bias, n_img, out=None, out_f32=None, in_img=Non
         if crop is not None:
             d.crop_top, d.crop_left = crop
             d.out_H, d.out_W = out_f32.shape[2], out_f32.shape[3]
-    if agg is not None:
-        feats, att, idx, N = agg
-        d.agg_feats, d.agg_n_img, d.agg_att, d.agg_N = feats.buf.data_ptr(), feats.n_img, att.data_ptr(), N
-        if idx is not None:
-            d.agg_idx = dev_i32(idx)
     nbytes = L.esr_conv_small_workspace_bytes(k, p)
     ws = torch.empty((max(nbytes, 1),), dtype=torch.uint8, device=w.device)
     d.workspace, d.workspace_bytes = ws.data_ptr(), nbytes

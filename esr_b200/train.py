@@ -17,7 +17,6 @@ plan and cannot be differentiated); DeepRecurrNet.forward dispatches here when g
 """
 import contextlib
 import math
-import os
 
 import torch
 import torch.nn.functional as F
@@ -592,9 +591,9 @@ def _step_body(model, optimizer, frames, gt, num_frame, all_reduce):
     optimizer.zero_grad()
     net = model.module if hasattr(model, "module") else model
     net.reset_states()
-    # the ConvGRU weight gradients are batched over all steps (one launch per gate; measured -1.5 ms per cfg2 iteration,
-    # ESR_TRAIN_DEFER=0 disables).  Not under DDP: its reducer must see every gradient inside backward.
-    defer = os.environ.get("ESR_TRAIN_DEFER", "1") == "1" and not hasattr(model, "module")
+    # the ConvGRU weight gradients are batched over all steps (one launch per gate; measured -1.5 ms per cfg2 iteration).
+    # Not under DDP: its reducer must see every gradient inside backward.
+    defer = not hasattr(model, "module")
     with _defer_weight_grads() if defer else contextlib.nullcontext() as deferred:
         pred = model(frames)                                      # all windows, window-major [(Wn*B), 2, H, W]
         target = gt[:, mid:mid + Wn].transpose(0, 1).reshape(pred.shape)

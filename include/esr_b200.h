@@ -172,28 +172,25 @@ int esr_split_to_nchw(const void *src, int n_img, int C, int H, int W, float *ds
 /* ---------------------------------------------------------------------------------------------
  * Small-channel and narrow-output convolutions, layer by layer (for tests and tools; the network launches the same kernels
  * from esr_net_forward).  One call runs one launch of the network's plan on a chosen kernel family:
- *   path 0 = warp-level tensor cores (mma.sync, split bf16), 1 = fp32 FFMA twins, 2 = the narrow-output CUDA-core kernels.
- * A (kind, path) pair the network never runs returns ESR_EUNSUPPORTED.
+ *   path 0 = warp-level tensor cores (mma.sync, split bf16), 1 = fp32 FFMA twins, 2 = the narrow-output CUDA-core kernel.
+ * A (kind, path) pair the network never runs, or an unknown kind, returns ESR_EUNSUPPORTED.
  *   kind             Cin -> Cout, stride, act; input; output                                       paths
  *   HEAD_ENC0        2 -> 8 relu (head, w_head / b_head) fused into 8 -> 16 stride 2 relu; fp32 NCHW [*, 2, H_in, W_in]
  *                    zero-padded by pad_* (CropSize); split out                                    0, 1
  *   ENC1 / ENC2      16 -> 32 / 32 -> 64, stride 2, relu; split in and out                         0, 1
- *   ATT32 / ATT16    32 -> 1 / 16 -> 1, sigmoid; split in; fp32 NHWC out [n_img, H_in, W_in, 1]    0, 1, 2
- *   RECON1 / RECON2  bilinear x2, then 32 -> 16 / 16 -> 8 relu; split in and out (2 H_in x 2 W_in);
- *                    agg_feats != NULL (path 0): the source is in + mean over n < agg_N of
- *                    agg_feats[agg_idx[img * agg_N + n]] * agg_att[same image and pixel]          0, 1
+ *   ATT32 / ATT16    32 -> 1 / 16 -> 1, sigmoid; split in; fp32 NHWC out [n_img, H_in, W_in, 1]    0, 1
+ *   RECON1 / RECON2  bilinear x2, then 32 -> 16 / 16 -> 8 relu; split in and out (2 H_in x 2 W_in) 0, 1
  *   TAIL             8 -> 2 relu; split in; fp32 NCHW out [n_img, 2, out_H, out_W] = the window at (crop_top, crop_left)
- *                    of the H_in x W_in result                                                     0, 1, 2
- *   PRED_MAP1 / ATTEN0  64 -> 1, 3x3, sigmoid; SPATIAL_KERNEL 64 -> 2, 1x1, sigmoid; split in; fp32 NHWC out   2
+ *                    of the H_in x W_in result                                                     0, 1
+ *   SPATIAL_KERNEL   64 -> 2, 1x1, sigmoid; split in; fp32 NHWC out [n_img, H_in, W_in, 2]         2
  * Weights are fp32 [Cout, Cin, k, k], packed into `workspace` (esr_conv_small_workspace_bytes(kind, path) bytes) on `stream` by
- * the network's own packers.  Split tensors are [2 planes][n_img][H][W][C] bf16; in_n_img / out_n_img / agg_n_img give the
- * images per plane.  in_img (optional, not with TAIL on path 2): output image -> input image.  Stride-2 outputs are
- * (H - 1) / 2 + 1 high for a conv input of H rows (H_in + pad_top + pad_bottom for HEAD_ENC0).
+ * the network's own packers.  Split tensors are [2 planes][n_img][H][W][C] bf16; in_n_img / out_n_img give the images per
+ * plane.  in_img (optional): output image -> input image.  Stride-2 outputs are (H - 1) / 2 + 1 high for a conv input of H rows
+ * (H_in + pad_top + pad_bottom for HEAD_ENC0).
  * --------------------------------------------------------------------------------------------- */
 enum {
     ESR_CONV_SMALL_HEAD_ENC0 = 0, ESR_CONV_SMALL_ENC1, ESR_CONV_SMALL_ENC2, ESR_CONV_SMALL_ATT32, ESR_CONV_SMALL_ATT16,
-    ESR_CONV_SMALL_RECON1, ESR_CONV_SMALL_RECON2, ESR_CONV_SMALL_TAIL, ESR_CONV_SMALL_PRED_MAP1, ESR_CONV_SMALL_ATTEN0,
-    ESR_CONV_SMALL_SPATIAL_KERNEL
+    ESR_CONV_SMALL_RECON1, ESR_CONV_SMALL_RECON2, ESR_CONV_SMALL_TAIL, ESR_CONV_SMALL_SPATIAL_KERNEL = 10
 };
 typedef struct esr_conv_small_desc {
     int kind, path;
@@ -208,7 +205,6 @@ typedef struct esr_conv_small_desc {
     void *out; int out_n_img;               /* split output */
     float *out_f32;                         /* fp32 output */
     int crop_top, crop_left, out_H, out_W;  /* TAIL */
-    const void *agg_feats; int agg_n_img; const float *agg_att; const int32_t *agg_idx; int agg_N;   /* RECON1 / RECON2 */
     void *workspace; size_t workspace_bytes;
 } esr_conv_small_desc;
 size_t esr_conv_small_workspace_bytes(int kind, int path);
@@ -300,7 +296,7 @@ int esr_net_reset_states(esr_net_t net, esr_stream_t stream);
 int esr_net_reset_sample_states(esr_net_t net, int b, esr_stream_t stream);
 int esr_net_forward(esr_net_t net, const float *input, const int32_t *in_img, float *output, esr_stream_t stream);
 /* Same as esr_net_forward, but brackets every kernel launch with CUDA events on `stream`, synchronises, and reports
- * per-launch {class (0 tensor-core conv, 1 CUDA-core conv, 2 element-wise/sampling, 3 cooperative ConvGRU chain),
+ * per-launch {class (0 tensor-core conv, 1 CUDA-core conv, 2 element-wise/sampling),
  * milliseconds, algorithmic FLOPs, algorithmic bytes (every input / output element once at 4 bytes), layer name (32 chars each)}
  * into host arrays (measurement aid for bench.py's roofline objects; not on the production path).  bytes_host / names_host
  * may be null. */
@@ -377,8 +373,7 @@ int esr_conv2d_backward(const float *x, const void *x_split, const float *w, con
                         size_t workspace_bytes, esr_stream_t stream);
 /* Replaces the same ATen conv2d backward (train_ops.cu, for a ConvLayer of models/submodules.py:159-200) with `flags`: 0 is
  * esr_conv2d_backward; ESR_DETERMINISTIC sums db and dw from per-block partials in a fixed order (what
- * torch.backends.cudnn.deterministic asks of cuDNN), with esr_conv2d_workspace_bytes_ex(..., flags) bytes of workspace.  The
- * opt-in ESR_WGRAD_MMA weight gradient has no deterministic variant: ESR_EUNSUPPORTED. */
+ * torch.backends.cudnn.deterministic asks of cuDNN), with esr_conv2d_workspace_bytes_ex(..., flags) bytes of workspace. */
 size_t esr_conv2d_workspace_bytes_ex(int B, int Cin, int H, int W, int Cout, int ksz, int stride, int flags);
 int esr_conv2d_backward_ex(const float *x, const void *x_split, const float *w, const float *y, const float *dy, int B, int Cin,
                            int H, int W, int Cout, int ksz, int stride, int act, float *dx, float *dw, float *db, int flags,

@@ -82,14 +82,11 @@ def test_tc_layer_deterministic_vs_fp64(dev, cudnn_det, monkeypatch, name):
     rep.again()
 
 
-NARROW = [n for n, c in sc.TRAIN_NARROW.items() if not c[9].get("wgrad_mma")]
-
-
-@pytest.mark.parametrize("name", NARROW)
+@pytest.mark.parametrize("name", list(sc.TRAIN_NARROW))
 def test_narrow_layer_deterministic_vs_fp64(dev, cudnn_det, monkeypatch, name):
     """k_conv_wgrad_r / k_conv_wgrad_g<1> (per-split partials + ordered sum) and k_bias_grad's partials."""
     rep = _repeat_conv(monkeypatch)
-    sc.test_train_narrow_conv2d_vs_fp64(dev, name, monkeypatch)
+    sc.test_train_narrow_conv2d_vs_fp64(dev, name)
     rep.again()
 
 
@@ -231,17 +228,6 @@ def test_deterministic_train_step_tracks_oracle_losses(dev, torch_det):
 
 
 # ------------------------------------------------------------------------------------------------------------------ errors
-def test_wgrad_mma_raises_in_deterministic_mode(dev, cudnn_det, monkeypatch):
-    from esr_b200 import _lib, train
-    monkeypatch.setenv("ESR_WGRAD_MMA", "1")
-    x = torch.randn(2, 16, 40, 50, device=dev, requires_grad=True)
-    w = torch.randn(8, 16, 3, 3, device=dev, requires_grad=True)
-    b = torch.zeros(8, device=dev, requires_grad=True)
-    y = train.conv2d(x, w, b, 1, "relu")
-    with pytest.raises(_lib.ESRError, match="ESR_WGRAD_MMA"):
-        y.sum().backward()
-
-
 def test_generic_dcn_backward_raises_in_deterministic_mode(dev, cudnn_det):
     """The reference's own DCN test configuration (2 -> 2 channels, 1 group) runs on the generic kernels: no deterministic
     variant."""

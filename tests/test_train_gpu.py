@@ -51,6 +51,10 @@ CONV_CASES = [
     (1, 32, 16, 3, 1, None, 70, 130),
     (1, 8, 2, 3, 1, "relu", 20, 64),            # exactly one tile wide
     (1, 64, 32, 3, 1, "relu", 20, 70),          # Cout 32: g padded to 64 channels for the tensor-core dx / dw
+    (2, 16, 8, 3, 1, "relu", 40, 50),           # more narrow layers whose dw runs on k_conv_wgrad_r
+    (1, 32, 16, 3, 1, "relu", 33, 47),
+    (1, 8, 16, 3, 2, "relu", 33, 45),
+    (1, 2, 8, 3, 1, "relu", 20, 36),
 ]
 
 
@@ -340,23 +344,6 @@ def test_deferred_gru_weight_gradients_equal_per_step(dev):
     for (n, pa), (_, pb) in zip(a.named_parameters(), b.named_parameters()):
         assert pb.grad is not None, n
         assert _rel(pb.grad, pa.grad.cpu()) <= 1e-4, n
-
-
-@pytest.mark.parametrize("B,Cin,Cout,stride,H,W", [(2, 16, 8, 1, 40, 50), (1, 32, 16, 1, 33, 47), (2, 8, 16, 2, 40, 56), (1, 2, 8, 1, 20, 36)])
-def test_opt_in_mma_weight_gradient(dev, monkeypatch, B, Cin, Cout, stride, H, W):
-    """ESR_WGRAD_MMA=1: dw of the narrow layers through mma.sync (kept as an experiment) gives the same gradients."""
-    from esr_b200 import train
-    monkeypatch.setenv("ESR_WGRAD_MMA", "1")
-    g = torch.Generator().manual_seed(Cin + Cout + H)
-    x = torch.randn(B, Cin, H, W, generator=g, requires_grad=True)
-    w = (torch.randn(Cout, Cin, 3, 3, generator=g) / (Cin * 9) ** 0.5).requires_grad_()
-    b = torch.zeros(Cout, requires_grad=True)
-    want = torch.relu(F.conv2d(x, w, b, stride=stride, padding=1))
-    dy = torch.randn(want.shape, generator=g)
-    want.backward(dy)
-    xg, wg, bg = (t.detach().to(dev).requires_grad_() for t in (x, w, b))
-    train.conv2d(xg, wg, bg, stride, "relu").backward(dy.to(dev))
-    assert _rel(wg.grad, w.grad) <= REL and _rel(xg.grad, x.grad) <= REL
 
 
 def test_adam_follows_a_torch_lr_scheduler_also_inside_the_graph(dev):
