@@ -454,24 +454,37 @@ int conv_mma(DirectKind kind, const DirectArgs &a, cudaStream_t st)
     return ESR_EINVAL;
 }
 
+// The fp32 NCHW instantiations of the training operators: MMA_CASE(Cin, Cout, stride, tile width, tile height)
+#define MMA_NCHW_CASES(MMA_CASE)                                                                                                   \
+    MMA_CASE(2, 8, 1, 32, 16) MMA_CASE(32, 16, 1, 32, 8) MMA_CASE(16, 8, 1, 32, 16) MMA_CASE(8, 2, 1, 32, 16)                      \
+    MMA_CASE(32, 1, 1, 32, 8) MMA_CASE(16, 1, 1, 32, 16)                                                                           \
+    MMA_CASE(16, 32, 1, 32, 16) MMA_CASE(8, 16, 1, 32, 16) MMA_CASE(1, 32, 1, 32, 16) MMA_CASE(1, 16, 1, 32, 16) MMA_CASE(1, 64, 1, 32, 8) \
+    MMA_CASE(8, 16, 2, 16, 16) MMA_CASE(16, 32, 2, 16, 8) MMA_CASE(32, 64, 2, 16, 8)
+
+bool conv_mma_nchw_ok(int Cin, int Cout, int stride, int act)
+{
+    if (act != ACT_NONE && act != ACT_RELU && act != ACT_SIGMOID) return false;
+#define MMA_CASE(ci, co, s, tw, th) if (Cin == ci && Cout == co && stride == s) return true;
+    MMA_NCHW_CASES(MMA_CASE)
+#undef MMA_CASE
+    return false;
+}
+
 // fp32 NCHW in / out (the training operators): y = act(conv3x3(x) + bias), stride 1 or 2, weights as a pack_mma_weight image.
-// ESR_EINVAL = no instantiation for this (Cin, Cout, stride).
 int conv_mma_nchw(const float *x, const void *w_img, const float *bias, int B, int Cin, int H, int W, int Cout, int stride, int act,
                   float *y, cudaStream_t st)
 {
+    ESR_REQUIRE(conv_mma_nchw_ok(Cin, Cout, stride, act), "conv_mma_nchw: no instantiation for %d -> %d, stride %d, act %d", Cin,
+                Cout, stride, act);
     DirectArgs a;
     a.in_f32 = x; a.Hin = H; a.Win = W; a.w_mma = w_img; a.bias = bias; a.act = act;
     a.n_img = B; a.Hout = (H + 2 - 3) / stride + 1; a.Wout = (W + 2 - 3) / stride + 1;
     a.out_f32 = y; a.out_H = a.Hout; a.out_W = a.Wout;
-    if (act != ACT_NONE && act != ACT_RELU && act != ACT_SIGMOID) return ESR_EINVAL;
 #define MMA_CASE(ci, co, s, tw, th) \
     if (Cin == ci && Cout == co && stride == s) return launch_mma<ci, co, s, false, FMT_NCHW_F32, FMT_NCHW_F32, tw, th>(a, st);
-    MMA_CASE(2, 8, 1, 32, 16) MMA_CASE(32, 16, 1, 32, 8) MMA_CASE(16, 8, 1, 32, 16) MMA_CASE(8, 2, 1, 32, 16)
-    MMA_CASE(32, 1, 1, 32, 8) MMA_CASE(16, 1, 1, 32, 16)
-    MMA_CASE(16, 32, 1, 32, 16) MMA_CASE(8, 16, 1, 32, 16) MMA_CASE(1, 32, 1, 32, 16) MMA_CASE(1, 16, 1, 32, 16) MMA_CASE(1, 64, 1, 32, 8)
-    MMA_CASE(8, 16, 2, 16, 16) MMA_CASE(16, 32, 2, 16, 8) MMA_CASE(32, 64, 2, 16, 8)
+    MMA_NCHW_CASES(MMA_CASE)
 #undef MMA_CASE
-    return ESR_EINVAL;
+    return ESR_EINVAL;                                                   // not reached: conv_mma_nchw_ok reads the same list
 }
 
 } // namespace esr

@@ -777,50 +777,38 @@ __global__ void __launch_bounds__(256) k_adam(float *__restrict__ p, const float
 // ------------------------------------------------------------------------------------------------------------------
 // host side
 // ------------------------------------------------------------------------------------------------------------------
-static inline bool tc_fwd_ok(int Cin, int Cout, int ksz, int stride) { return stride == 1 && Cin % 64 == 0 && Cout <= 256 && (ksz == 3 || ksz == 1); }
-// dx / dw on the tensor cores: g is padded to a 64-multiple of channels; not worth it for the 1-, 2-, 8- and 16-channel layers
-static inline bool tc_dgrad_ok(int Cin, int Cout, int ksz, int stride) { return stride == 1 && Cout >= 32 && Cout <= 256 && Cin <= 256 && (ksz == 3 || ksz == 1); }
 static inline int pad64(int c) { return (c + 63) / 64 * 64; }
 
-static size_t conv2d_ws(int B, int Cin, int H, int W, int Cout, int ksz, int stride)
-{
-    const int Ho = (H + 2 * (ksz / 2) - ksz) / stride + 1, Wo = (W + 2 * (ksz / 2) - ksz) / stride + 1;
-    Bump f{nullptr, 0, 0}, b{nullptr, 0, 0};
-    if (tc_fwd_ok(Cin, Cout, ksz, stride)) {
-        f.take((size_t)B * Cin * H * W * 4); f.take(tc_packed_weight_bytes(Cout, Cin, ksz * ksz)); f.take(256 * 4);
-        f.take((size_t)B * tc_npad(Cout) * H * W * 4);
-    }
-    b.take((size_t)B * Cout * Ho * Wo * 4);
-    b.take((size_t)Cout * Cin * ksz * ksz * 4);                          // rotated weights of the CUDA-core dx path
-    b.take(mma_weight_bytes(Cin, Cout)); f.take(mma_weight_bytes(Cout, Cin));   // weight images of the mma.sync kernels
-    if (tc_dgrad_ok(Cin, Cout, ksz, stride)) {
-        b.take((size_t)B * pad64(Cout) * Ho * Wo * 4); b.take((size_t)B * Cin * H * W * 4);      // g split, x split (dw on tensor cores)
-        b.take((size_t)pad64(Cout) * Cin * ksz * ksz * 4);
-        b.take(tc_packed_weight_bytes(Cin, pad64(Cout), ksz * ksz)); b.take(256 * 4); b.take((size_t)B * tc_npad(Cin) * H * W * 4);
-    }
-    return (f.off > b.off ? f.off : b.off) + 1024;
-}
+// mma_conv.cu: conv_mma_nchw has an instantiation for (Cin, Cout, stride, act)
+bool conv_mma_nchw_ok(int Cin, int Cout, int stride, int act);
 
-// y = act(conv(x)) on the tensor cores: fp32 NCHW -> split NHWC -> k_conv_tc -> fp32 NCHW
-static int conv_tc_nchw(const float *x, const float *w, const float *bias, int B, int Cin, int H, int W, int Cout, int ksz, int act,
-                        float *y, void *x_split_out, Bump &ws, cudaStream_t st)
+// The kernels of one training convolution.  conv2d_paths is the one rule that picks them: the forward and backward entry
+// points, the workspace queries and esr_conv2d_split_bytes all ask it.
+enum ConvFwd { FWD_TC, FWD_MMA, FWD_R, FWD_G };           // k_conv_tc, k_conv_mma, k_conv_fwd_r, k_conv_fwd_g<k>
+enum ConvDx { DX_TC, DX_MMA, DX_R, DX_S2, DX_G };         // k_conv_tc over g, k_conv_mma, k_conv_fwd_r, k_conv_dgrad_s2 / _g<k>
+struct ConvPaths {
+    ConvFwd fwd;
+    ConvDx dx;                                            // DX_TC: g also goes to the split bf16 format (k_to_split)
+    bool tc_dw;                                           // k_wgrad_tc; otherwise k_conv_wgrad_r (3x3) / k_conv_wgrad_g<1>
+    bool det;                                             // ESR_DETERMINISTIC: the _det dw / db kernels, then k_sum_slices
+};
+
+static ConvPaths conv2d_paths(int Cin, int Cout, int ksz, int stride, int act, int flags)
 {
-    int rc;
-    SplitTensor xs; xs.n_img = B; xs.H = H; xs.W = W; xs.C = Cin;
-    xs.base = (__nv_bfloat16 *)(x_split_out ? x_split_out : ws.take((size_t)B * Cin * H * W * 4));   // kept by the caller for dw
-    void *wp = ws.take(tc_packed_weight_bytes(Cout, Cin, ksz * ksz));
-    float *bp = (float *)ws.take(256 * 4);
-    ESR_REQUIRE(ws.off <= ws.cap, "conv2d: workspace too small (%zu > %zu)", ws.off, ws.cap);
-    if ((rc = split_from_nchw_pad(x, B, Cin, Cin, H * W, xs.base, st))) return rc;
-    if ((rc = pack_conv_weight(w, Cout, Cin, ksz, wp, st))) return rc;
-    ESR_CUDA_CHECK(cudaMemsetAsync(bp, 0, 256 * 4, st));
-    if (bias) ESR_CUDA_CHECK(cudaMemcpyAsync(bp, bias, (size_t)Cout * 4, cudaMemcpyDeviceToDevice, st));
-    ConvTCDesc d;
-    d.src[0] = xs; d.n_src = 1; d.ntaps = ksz * ksz; d.cout = Cout; d.wpacked = wp; d.bias = bp; d.n_img = B; d.act = act;
-    d.out_f32 = y; d.out_f32_C = Cout; d.out_f32_nchw = 1;              // the epilogue writes fp32 NCHW directly
-    ConvTCArgs a;
-    if ((rc = conv_tc_prepare(d, &a))) return rc;
-    return conv_tc_launch(a, st);
+    static const bool no_mma = getenv("ESR_TRAIN_NO_MMA") != nullptr;
+    const bool k13 = ksz == 3 || ksz == 1;
+    // dx / dw on the tensor cores: g is padded to a 64-multiple of channels; not worth it for the 1-, 2-, 8- and 16-channel layers
+    const bool tc_dgrad = stride == 1 && Cout >= 32 && Cout <= 256 && Cin <= 256 && k13;
+    ConvPaths p;
+    if (stride == 1 && Cin % 64 == 0 && Cout <= 256 && k13) p.fwd = FWD_TC;
+    else if (ksz == 3 && !no_mma && conv_mma_nchw_ok(Cin, Cout, stride, act)) p.fwd = FWD_MMA;
+    else p.fwd = ksz == 3 && stride == 1 ? FWD_R : FWD_G;
+    if (tc_dgrad) p.dx = DX_TC;
+    else if (ksz == 3 && stride == 1) p.dx = !no_mma && conv_mma_nchw_ok(Cout, Cin, 1, ACT_NONE) ? DX_MMA : DX_R;
+    else p.dx = ksz == 3 ? DX_S2 : DX_G;
+    p.tc_dw = tc_dgrad && Cin % 64 == 0;
+    p.det = (flags & ESR_DETERMINISTIC) != 0;
+    return p;
 }
 
 // work slices (gridDim.y) of the CUDA-core weight-gradient kernels: about 8 blocks per SM, at most one per (image, tile) item
@@ -836,80 +824,143 @@ static int wgrad_slices(int B, int Cin, int Cout, int Ho, int Wo)
 // partial slots of the deterministic variant: per block, one per pixel split of k_conv_wgrad_r (3x3) / k_conv_wgrad_g<1> (1x1)
 static inline int wgrad_nsplit(int ksz) { return ksz == 3 ? WR_NSPLIT : 256 / G_C; }
 
-// which: 0 forward, 1 dx, 2 dw.  part (dw only): deterministic mode -- partials go to part, then an ordered sum into out.
-template <int KS>
-static int launch_generic(int which, const float *x, const float *w, const float *bias, const float *g, float *out, int B, int Cin,
-                          int H, int W, int Cout, int Ho, int Wo, int stride, int act, cudaStream_t st, float *part = nullptr)
+// wgrad_tc.cu.  part != NULL: deterministic (see wgrad_tc_part_bytes)
+int wgrad_tc(const __nv_bfloat16 *x_split, const __nv_bfloat16 *g_split, int B, int Cin, int H, int W, int Cout, int CoutPad, int ksz,
+             float *dw, float *part, cudaStream_t st);
+size_t wgrad_tc_part_bytes(int B, int Cin, int H, int W, int Cout, int CoutPad, int ksz);
+
+// Byte offsets of every buffer of one training convolution in its workspace, and the size the workspace queries report.
+// The forward and the backward are separate calls, so each lays its buffers out from offset 0.
+struct Conv2dLayout {
+    size_t f_x_split, f_w_tc, f_bias, f_w_mma;            // forward: x split (when the caller keeps none), weight image, bias
+    size_t g, g_split, x_split, wt, w_tc, bias, w_mma;    // backward: g in fp32 / split, x split for dw, the weights of dx
+    size_t bias_part, dw_part;                            // backward, deterministic mode: the partials k_sum_slices adds
+    size_t total;
+};
+
+static Conv2dLayout conv2d_layout(int B, int Cin, int H, int W, int Cout, int ksz, int stride, const ConvPaths &p)
 {
-    constexpr int KK = KS * KS;
-    const dim3 blk(G_T, G_T);
-    if (which == 2 && part) {
-        const int PD = (G_T - 1) * stride + KS;
-        const size_t smem = (size_t)(256 * G_C + G_C * PD * PD) * 4;
-        const int pairs = ((Cout + G_C - 1) / G_C) * ((Cin + G_C - 1) / G_C);
-        const int slices = wgrad_slices(B, Cin, Cout, Ho, Wo);
-        static bool attr = false;
-        if constexpr (KS == 3) {
-            if (!attr) { ESR_CUDA_CHECK(cudaFuncSetAttribute(k_conv_wgrad_r_det, cudaFuncAttributeMaxDynamicSharedMemorySize, 64 * 1024)); attr = true; }
-            k_conv_wgrad_r_det<<<dim3(pairs, slices), 256, smem, st>>>(x, g, part, B, Cin, H, W, Cout, Ho, Wo, stride);
-        } else {
-            if (!attr) { ESR_CUDA_CHECK(cudaFuncSetAttribute(k_conv_wgrad_g_det<KS>, cudaFuncAttributeMaxDynamicSharedMemorySize, 64 * 1024)); attr = true; }
-            k_conv_wgrad_g_det<KS><<<dim3(pairs, slices), 256, smem, st>>>(x, g, part, B, Cin, H, W, Cout, Ho, Wo, stride);
-        }
-        ESR_LAUNCH_CHECK();
-        return sum_slices(part, slices * wgrad_nsplit(KS), (size_t)Cout * Cin * KK, out, st);
+    const int Ho = (H + 2 * (ksz / 2) - ksz) / stride + 1, Wo = (W + 2 * (ksz / 2) - ksz) / stride + 1;
+    const int KK = ksz * ksz, gC = pad64(Cout);
+    const size_t x_bytes = (size_t)B * Cin * H * W * 4;
+    Conv2dLayout l{};
+    size_t off = 0;
+    auto take = [&](size_t bytes) { size_t r = off; off = align_up(off + bytes, 256); return r; };
+    if (p.fwd == FWD_TC) {
+        l.f_x_split = take(x_bytes); l.f_w_tc = take(tc_packed_weight_bytes(Cout, Cin, KK)); l.f_bias = take(256 * 4);
+    } else if (p.fwd == FWD_MMA) {
+        l.f_w_mma = take(mma_weight_bytes(Cout, Cin));
     }
-    if (which == 0 && KS == 3 && stride == 1) {
+    const size_t fwd_end = off;
+    off = 0;
+    l.g = take((size_t)B * Cout * Ho * Wo * 4);                       // fp32 g: only the CUDA-core kernels read it
+    if (p.dx == DX_TC) {
+        l.g_split = take((size_t)B * gC * Ho * Wo * 4);
+        // the x split that dw converts when the caller kept none is dead before dx: the weights of dx reuse its space
+        l.x_split = off;
+        l.wt = take((size_t)gC * Cin * KK * 4); l.w_tc = take(tc_packed_weight_bytes(Cin, gC, KK)); l.bias = take(256 * 4);
+        if (p.tc_dw && off < align_up(l.x_split + x_bytes, 256)) off = align_up(l.x_split + x_bytes, 256);
+    } else if (p.dx == DX_MMA) {
+        l.w_mma = take(mma_weight_bytes(Cin, Cout));
+    } else if (p.dx == DX_R) {
+        l.wt = take((size_t)Cout * Cin * 9 * 4);
+    }
+    if (p.det) {
+        l.bias_part = take((size_t)64 * Cout * 4);                    // <= 64 chunks of bias_grad
+        l.dw_part = take(p.tc_dw ? wgrad_tc_part_bytes(B, Cin, H, W, Cout, gC, ksz)
+                                 : (size_t)wgrad_slices(B, Cin, Cout, Ho, Wo) * wgrad_nsplit(ksz) * Cout * Cin * KK * 4);
+    }
+    l.total = fwd_end > off ? fwd_end : off;
+    return l;
+}
+
+// fp32 NCHW output of k_conv_tc: out = act(conv(src, wp) + bias), bias padded to 256 channels
+static int conv_tc_to_nchw(const SplitTensor &src, int ntaps, int cout, const void *wp, const float *bias, int act, float *out,
+                           cudaStream_t st)
+{
+    ConvTCDesc d;
+    d.src[0] = src; d.n_src = 1; d.ntaps = ntaps; d.cout = cout; d.wpacked = wp; d.bias = bias; d.n_img = src.n_img; d.act = act;
+    d.out_f32 = out; d.out_f32_C = cout; d.out_f32_nchw = 1;           // the epilogue writes fp32 NCHW directly
+    ConvTCArgs a;
+    int rc;
+    if ((rc = conv_tc_prepare(d, &a))) return rc;
+    return conv_tc_launch(a, st);
+}
+
+// ---- the CUDA-core launchers; kernels with more than 48 KB of shared memory are opted in at their first launch
+
+// FWD_R (3x3, stride 1) or FWD_G
+template <int KS>
+static int launch_fwd(ConvFwd k, const float *x, const float *w, const float *bias, float *y, int B, int Cin, int H, int W, int Cout,
+                      int Ho, int Wo, int stride, int act, cudaStream_t st)
+{
+    if (k == FWD_R) {
         const size_t smem = (size_t)(G_C * R_PH * R_PW + G_C * 9 * G_C) * 4;
         const dim3 grid(((Wo + R_TW - 1) / R_TW) * ((Ho + R_TH - 1) / R_TH), (Cout + G_C - 1) / G_C, B);
-        k_conv_fwd_r<<<grid, 256, smem, st>>>(x, w, bias, out, Cin, H, W, Cout, act);
-    } else if (which == 2 && KS == 3) {
-        const int PD = (G_T - 1) * stride + 3;
-        const size_t smem = (size_t)(256 * G_C + G_C * PD * PD) * 4;
-        const int pairs = ((Cout + G_C - 1) / G_C) * ((Cin + G_C - 1) / G_C);
-        const int items = B * ((Wo + G_T - 1) / G_T) * ((Ho + G_T - 1) / G_T);
-        int slices = (dev_info().sm_count * 8 + pairs - 1) / pairs;
-        if (slices > items) slices = items;
-        if (slices < 1) slices = 1;
-        static bool attr = false;
-        if (!attr) { ESR_CUDA_CHECK(cudaFuncSetAttribute(k_conv_wgrad_r, cudaFuncAttributeMaxDynamicSharedMemorySize, 64 * 1024)); attr = true; }
-        k_conv_wgrad_r<<<dim3(pairs, slices), 256, smem, st>>>(x, g, out, B, Cin, H, W, Cout, Ho, Wo, stride);
-    } else if (which == 0) {
+        k_conv_fwd_r<<<grid, 256, smem, st>>>(x, w, bias, y, Cin, H, W, Cout, act);
+    } else {
         const int PD = (G_T - 1) * stride + KS;
-        const size_t smem = (size_t)(G_C * PD * PD + G_C * G_C * KK) * 4;
+        const size_t smem = (size_t)(G_C * PD * PD + G_C * G_C * KS * KS) * 4;
         const dim3 grid(((Wo + G_T - 1) / G_T) * ((Ho + G_T - 1) / G_T), (Cout + G_C - 1) / G_C, B);
         static bool attr = false;
         if (!attr) { ESR_CUDA_CHECK(cudaFuncSetAttribute(k_conv_fwd_g<KS>, cudaFuncAttributeMaxDynamicSharedMemorySize, 64 * 1024)); attr = true; }
-        k_conv_fwd_g<KS><<<grid, blk, smem, st>>>(x, w, bias, out, Cin, H, W, Cout, Ho, Wo, stride, act);
-    } else if (which == 1 && KS == 3 && stride == 2) {
-        const dim3 grid(((W + 31) / 32) * ((H + 31) / 32), (Cin + G_C - 1) / G_C, B);
-        k_conv_dgrad_s2<<<grid, 256, 0, st>>>(g, w, out, Cin, H, W, Cout, Ho, Wo);
-    } else if (which == 1) {
-        const int GP = (G_T - 1 + KS - 1) / stride + 2;
-        const size_t smem = (size_t)(G_C * GP * GP + G_C * G_C * KK) * 4;
-        const dim3 grid(((W + G_T - 1) / G_T) * ((H + G_T - 1) / G_T), (Cin + G_C - 1) / G_C, B);
-        k_conv_dgrad_g<KS><<<grid, blk, smem, st>>>(g, w, out, Cin, H, W, Cout, Ho, Wo, stride);
-    } else {
-        const int PD = (G_T - 1) * stride + KS;
-        const size_t smem = (size_t)(256 * G_C + G_C * PD * PD) * 4;
-        const int pairs = ((Cout + G_C - 1) / G_C) * ((Cin + G_C - 1) / G_C);
-        const int items = B * ((Wo + G_T - 1) / G_T) * ((Ho + G_T - 1) / G_T);
-        int slices = (dev_info().sm_count * 8 + pairs - 1) / pairs;
-        if (slices > items) slices = items;
-        if (slices < 1) slices = 1;
-        static bool attr = false;
-        if (!attr) { ESR_CUDA_CHECK(cudaFuncSetAttribute(k_conv_wgrad_g<KS>, cudaFuncAttributeMaxDynamicSharedMemorySize, 64 * 1024)); attr = true; }
-        k_conv_wgrad_g<KS><<<dim3(pairs, slices), 256, smem, st>>>(x, g, out, B, Cin, H, W, Cout, Ho, Wo, stride);
+        k_conv_fwd_g<KS><<<grid, dim3(G_T, G_T), smem, st>>>(x, w, bias, y, Cin, H, W, Cout, Ho, Wo, stride, act);
     }
     ESR_LAUNCH_CHECK();
     return ESR_OK;
 }
 
-static int generic(int which, int ksz, const float *x, const float *w, const float *bias, const float *g, float *out, int B, int Cin,
-                   int H, int W, int Cout, int Ho, int Wo, int stride, int act, cudaStream_t st, float *part = nullptr)
+// DX_S2 or DX_G
+template <int KS>
+static int launch_dx(ConvDx k, const float *g, const float *w, float *dx, int B, int Cin, int H, int W, int Cout, int Ho, int Wo,
+                     int stride, cudaStream_t st)
 {
-    return ksz == 3 ? launch_generic<3>(which, x, w, bias, g, out, B, Cin, H, W, Cout, Ho, Wo, stride, act, st, part)
-                    : launch_generic<1>(which, x, w, bias, g, out, B, Cin, H, W, Cout, Ho, Wo, stride, act, st, part);
+    if (k == DX_S2) {
+        const dim3 grid(((W + 31) / 32) * ((H + 31) / 32), (Cin + G_C - 1) / G_C, B);
+        k_conv_dgrad_s2<<<grid, 256, 0, st>>>(g, w, dx, Cin, H, W, Cout, Ho, Wo);
+    } else {
+        const int GP = (G_T - 1 + KS - 1) / stride + 2;
+        const size_t smem = (size_t)(G_C * GP * GP + G_C * G_C * KS * KS) * 4;
+        const dim3 grid(((W + G_T - 1) / G_T) * ((H + G_T - 1) / G_T), (Cin + G_C - 1) / G_C, B);
+        k_conv_dgrad_g<KS><<<grid, dim3(G_T, G_T), smem, st>>>(g, w, dx, Cin, H, W, Cout, Ho, Wo, stride);
+    }
+    ESR_LAUNCH_CHECK();
+    return ESR_OK;
+}
+
+// k_conv_wgrad_r (3x3) / k_conv_wgrad_g<1> adding into dw; part != NULL: deterministic -- the _det kernel writes its partials
+// to part, then k_sum_slices adds them into dw in slot order
+template <int KS>
+static int launch_dw(const float *x, const float *g, float *dw, float *part, int B, int Cin, int H, int W, int Cout, int Ho, int Wo,
+                     int stride, cudaStream_t st)
+{
+    const int PD = (G_T - 1) * stride + KS;
+    const size_t smem = (size_t)(256 * G_C + G_C * PD * PD) * 4;
+    const int pairs = ((Cout + G_C - 1) / G_C) * ((Cin + G_C - 1) / G_C);
+    const int slices = wgrad_slices(B, Cin, Cout, Ho, Wo);
+    const dim3 grid(pairs, slices);
+    if (part) {
+        static bool attr = false;
+        if constexpr (KS == 3) {
+            if (!attr) { ESR_CUDA_CHECK(cudaFuncSetAttribute(k_conv_wgrad_r_det, cudaFuncAttributeMaxDynamicSharedMemorySize, 64 * 1024)); attr = true; }
+            k_conv_wgrad_r_det<<<grid, 256, smem, st>>>(x, g, part, B, Cin, H, W, Cout, Ho, Wo, stride);
+        } else {
+            if (!attr) { ESR_CUDA_CHECK(cudaFuncSetAttribute(k_conv_wgrad_g_det<KS>, cudaFuncAttributeMaxDynamicSharedMemorySize, 64 * 1024)); attr = true; }
+            k_conv_wgrad_g_det<KS><<<grid, 256, smem, st>>>(x, g, part, B, Cin, H, W, Cout, Ho, Wo, stride);
+        }
+        ESR_LAUNCH_CHECK();
+        return sum_slices(part, slices * wgrad_nsplit(KS), (size_t)Cout * Cin * KS * KS, dw, st);
+    }
+    static bool attr = false;
+    if (KS == 3) {
+        if (!attr) { ESR_CUDA_CHECK(cudaFuncSetAttribute(k_conv_wgrad_r, cudaFuncAttributeMaxDynamicSharedMemorySize, 64 * 1024)); attr = true; }
+        k_conv_wgrad_r<<<grid, 256, smem, st>>>(x, g, dw, B, Cin, H, W, Cout, Ho, Wo, stride);
+    } else {
+        if (!attr) { ESR_CUDA_CHECK(cudaFuncSetAttribute(k_conv_wgrad_g<KS>, cudaFuncAttributeMaxDynamicSharedMemorySize, 64 * 1024)); attr = true; }
+        k_conv_wgrad_g<KS><<<grid, 256, smem, st>>>(x, g, dw, B, Cin, H, W, Cout, Ho, Wo, stride);
+    }
+    ESR_LAUNCH_CHECK();
+    return ESR_OK;
 }
 
 // db = sum of g over (image, pixel); part != NULL: deterministic (per-block partials, then the ordered sum)
@@ -928,28 +979,6 @@ static int bias_grad(const float *g, int B, int Cout, int HW, float *db, float *
     return sum_slices(part, chunks, (size_t)Cout, db, st);
 }
 
-// wgrad_tc.cu (returns ESR_EINVAL when the shape is not supported).  part != NULL: deterministic (see wgrad_tc_part_bytes)
-int wgrad_tc(const __nv_bfloat16 *x_split, const __nv_bfloat16 *g_split, int B, int Cin, int H, int W, int Cout, int CoutPad, int ksz,
-             float *dw, float *part, cudaStream_t st);
-size_t wgrad_tc_part_bytes(int B, int Cin, int H, int W, int Cout, int CoutPad, int ksz);
-
-// the dw kernel esr_conv2d_backward picks: k_wgrad_tc for the 64-multiple layers, the CUDA-core kernels otherwise
-static inline bool use_tc_dw(int Cin, int Cout, int ksz, int stride)
-{
-    return tc_dgrad_ok(Cin, Cout, ksz, stride) && Cin % 64 == 0 && getenv("ESR_WGRAD_GENERIC") == nullptr;
-}
-
-// deterministic mode's extra workspace, after the default layout: bias partials (<= 64 chunks), then the dw partials
-static size_t conv2d_det_bias_bytes(int Cout) { return align_up((size_t)64 * Cout * 4, 256); }
-static size_t conv2d_det_bytes(int B, int Cin, int H, int W, int Cout, int ksz, int stride)
-{
-    const int Ho = (H + 2 * (ksz / 2) - ksz) / stride + 1, Wo = (W + 2 * (ksz / 2) - ksz) / stride + 1;
-    const size_t dw = use_tc_dw(Cin, Cout, ksz, stride)
-                          ? wgrad_tc_part_bytes(B, Cin, H, W, Cout, pad64(Cout), ksz)
-                          : (size_t)wgrad_slices(B, Cin, Cout, Ho, Wo) * wgrad_nsplit(ksz) * Cout * Cin * ksz * ksz * 4;
-    return conv2d_det_bias_bytes(Cout) + dw;
-}
-
 } // namespace esr
 
 using namespace esr;
@@ -958,19 +987,19 @@ extern "C" {
 
 size_t esr_conv2d_workspace_bytes(int B, int Cin, int H, int W, int Cout, int ksz, int stride)
 {
-    return conv2d_ws(B, Cin, H, W, Cout, ksz, stride);
+    return esr_conv2d_workspace_bytes_ex(B, Cin, H, W, Cout, ksz, stride, 0);
 }
 
+// The queries take no activation: they size for one that the mma kernels serve (tanh only drops the forward's mma weights).
 size_t esr_conv2d_workspace_bytes_ex(int B, int Cin, int H, int W, int Cout, int ksz, int stride, int flags)
 {
-    const size_t base = conv2d_ws(B, Cin, H, W, Cout, ksz, stride);
-    return (flags & ESR_DETERMINISTIC) ? base + conv2d_det_bytes(B, Cin, H, W, Cout, ksz, stride) : base;
+    return conv2d_layout(B, Cin, H, W, Cout, ksz, stride, conv2d_paths(Cin, Cout, ksz, stride, ACT_NONE, flags)).total;
 }
 
 size_t esr_conv2d_split_bytes(int B, int Cin, int H, int W, int Cout, int ksz, int stride)
 {
-    const bool both = tc_fwd_ok(Cin, Cout, ksz, stride) && tc_dgrad_ok(Cin, Cout, ksz, stride) && Cin % 64 == 0;
-    return both ? (size_t)B * Cin * H * W * 4 : 0;
+    const ConvPaths p = conv2d_paths(Cin, Cout, ksz, stride, ACT_NONE, 0);
+    return p.fwd == FWD_TC && p.tc_dw ? (size_t)B * Cin * H * W * 4 : 0;
 }
 
 int esr_conv2d_forward(const float *x, const float *w, const float *bias, int B, int Cin, int H, int W, int Cout, int ksz, int stride,
@@ -982,20 +1011,29 @@ int esr_conv2d_forward(const float *x, const float *w, const float *bias, int B,
                 stride, act);
     ESR_REQUIRE(B > 0 && Cin > 0 && Cout > 0 && H > 0 && W > 0, "conv2d_forward: bad shape");
     const int pad = ksz / 2, Ho = (H + 2 * pad - ksz) / stride + 1, Wo = (W + 2 * pad - ksz) / stride + 1;
-    if (tc_fwd_ok(Cin, Cout, ksz, stride)) {
-        ESR_REQUIRE(workspace, "conv2d_forward: workspace required");
-        Bump ws{(uint8_t *)workspace, 0, workspace_bytes};
-        return conv_tc_nchw(x, w, bias, B, Cin, H, W, Cout, ksz, act, y, x_split_out, ws, st);
+    const ConvPaths p = conv2d_paths(Cin, Cout, ksz, stride, act, 0);
+    const Conv2dLayout L = conv2d_layout(B, Cin, H, W, Cout, ksz, stride, p);
+    ESR_REQUIRE(workspace && workspace_bytes >= L.total, "conv2d_forward: workspace of %zu bytes (%p), %zu needed", workspace_bytes,
+                workspace, L.total);
+    uint8_t *ws = (uint8_t *)workspace;
+    int rc;
+    if (p.fwd == FWD_TC) {
+        SplitTensor xs; xs.n_img = B; xs.H = H; xs.W = W; xs.C = Cin;
+        xs.base = (__nv_bfloat16 *)(x_split_out ? x_split_out : ws + L.f_x_split);   // kept by the caller for dw
+        float *bp = (float *)(ws + L.f_bias);
+        if ((rc = split_from_nchw_pad(x, B, Cin, Cin, H * W, xs.base, st))) return rc;
+        if ((rc = pack_conv_weight(w, Cout, Cin, ksz, ws + L.f_w_tc, st))) return rc;
+        ESR_CUDA_CHECK(cudaMemsetAsync(bp, 0, 256 * 4, st));
+        ESR_CUDA_CHECK(cudaMemcpyAsync(bp, bias, (size_t)Cout * 4, cudaMemcpyDeviceToDevice, st));
+        return conv_tc_to_nchw(xs, ksz * ksz, Cout, ws + L.f_w_tc, bp, act, y, st);
     }
-    static const bool no_mma = getenv("ESR_TRAIN_NO_MMA") != nullptr;
-    if (ksz == 3 && !no_mma && workspace && workspace_bytes >= mma_weight_bytes(Cout, Cin)) {
+    if (p.fwd == FWD_MMA) {
         // narrow layers: warp-level tensor cores (mma_conv.cu) on fp32 NCHW; weights packed to the split-bf16 image first
-        int rc = pack_mma_weight(w, Cout, Cin, workspace, st);
-        if (rc) return rc;
-        rc = conv_mma_nchw(x, workspace, bias, B, Cin, H, W, Cout, stride, act, y, st);
-        if (rc != ESR_EINVAL) return rc;
+        if ((rc = pack_mma_weight(w, Cout, Cin, ws + L.f_w_mma, st))) return rc;
+        return conv_mma_nchw(x, ws + L.f_w_mma, bias, B, Cin, H, W, Cout, stride, act, y, st);
     }
-    return generic(0, ksz, x, w, bias, nullptr, y, B, Cin, H, W, Cout, Ho, Wo, stride, act, st);
+    return ksz == 3 ? launch_fwd<3>(p.fwd, x, w, bias, y, B, Cin, H, W, Cout, Ho, Wo, stride, act, st)
+                    : launch_fwd<1>(p.fwd, x, w, bias, y, B, Cin, H, W, Cout, Ho, Wo, stride, act, st);
 }
 
 int esr_conv2d_backward(const float *x, const void *x_split, const float *w, const float *y, const float *dy, int B, int Cin, int H,
@@ -1011,49 +1049,40 @@ int esr_conv2d_backward_ex(const float *x, const void *x_split, const float *w, 
                            size_t workspace_bytes, esr_stream_t stream)
 {
     cudaStream_t st = (cudaStream_t)stream;
-    ESR_REQUIRE((x || x_split) && w && dy && workspace && ((dw && db) || (!dw && !db && dx)), "conv2d_backward: null pointer");
-    ESR_REQUIRE(!x_split || esr_conv2d_split_bytes(B, Cin, H, W, Cout, ksz, stride) > 0, "conv2d_backward: x_split given for a layer without a tensor-core dw");
-    ESR_REQUIRE(x || getenv("ESR_WGRAD_GENERIC") == nullptr, "conv2d_backward: the CUDA-core dw needs x");
-    const bool want_dw = dw != nullptr;                               // dw == db == NULL: input gradient only (deferred dw)
+    ESR_REQUIRE((x || x_split) && w && dy && ((dw && db) || (!dw && !db && dx)), "conv2d_backward: null pointer");
     ESR_REQUIRE(act == ACT_NONE || y, "conv2d_backward: the forward output is needed for the activation derivative");
     ESR_REQUIRE((ksz == 3 || ksz == 1) && (stride == 1 || stride == 2) && act >= 0 && act <= 3, "conv2d_backward: ksz=%d stride=%d act=%d", ksz,
                 stride, act);
     const int pad = ksz / 2, Ho = (H + 2 * pad - ksz) / stride + 1, Wo = (W + 2 * pad - ksz) / stride + 1;
-    // deterministic mode: the partial buffers sit after the default layout (esr_conv2d_workspace_bytes_ex)
-    const bool det = (flags & ESR_DETERMINISTIC) != 0;
-    const size_t base_bytes = conv2d_ws(B, Cin, H, W, Cout, ksz, stride);
-    float *bias_part = nullptr, *dw_part = nullptr;
-    if (det && want_dw) {
-        ESR_REQUIRE(workspace_bytes >= base_bytes + conv2d_det_bytes(B, Cin, H, W, Cout, ksz, stride),
-                    "conv2d_backward: deterministic mode needs esr_conv2d_workspace_bytes_ex(..., ESR_DETERMINISTIC) bytes");
-        bias_part = (float *)((uint8_t *)workspace + base_bytes);
-        dw_part = (float *)((uint8_t *)workspace + base_bytes + conv2d_det_bias_bytes(Cout));
-    }
-    Bump ws{(uint8_t *)workspace, 0, det ? base_bytes : workspace_bytes};
+    const ConvPaths p = conv2d_paths(Cin, Cout, ksz, stride, act, flags);
+    ESR_REQUIRE(!x_split || p.tc_dw, "conv2d_backward: x_split given for a layer without a tensor-core dw");
+    const bool want_dw = dw != nullptr;                               // dw == db == NULL: input gradient only (deferred dw)
+    ESR_REQUIRE(!want_dw || x || (p.tc_dw && x_split), "conv2d_backward: dw needs x (or, on the tensor cores, the forward's x_split)");
+    const Conv2dLayout L = conv2d_layout(B, Cin, H, W, Cout, ksz, stride, p);
+    ESR_REQUIRE(workspace && workspace_bytes >= L.total, "conv2d_backward: workspace of %zu bytes (%p), %zu needed", workspace_bytes,
+                workspace, L.total);
+    uint8_t *ws = (uint8_t *)workspace;
+    float *bias_part = p.det && want_dw ? (float *)(ws + L.bias_part) : nullptr;
+    float *dw_part = p.det && want_dw ? (float *)(ws + L.dw_part) : nullptr;
     int rc;
     const size_t ng = (size_t)B * Cout * Ho * Wo;
-    const bool tcd = tc_dgrad_ok(Cin, Cout, ksz, stride);
     const int gC = pad64(Cout);
-    const bool tc_dw = tcd && use_tc_dw(Cin, Cout, ksz, stride);
-    float *g = (float *)ws.take(ng * 4);                           // fp32 g: only the CUDA-core kernels read it
-    __nv_bfloat16 *gsplit = nullptr;
+    float *g = (float *)(ws + L.g);
+    __nv_bfloat16 *gsplit = (__nv_bfloat16 *)(ws + L.g_split);
     if (want_dw) {
         ESR_CUDA_CHECK(cudaMemsetAsync(db, 0, (size_t)Cout * 4, st));
         ESR_CUDA_CHECK(cudaMemsetAsync(dw, 0, (size_t)Cout * Cin * ksz * ksz * 4, st));
     }
-    if (tcd) {
+    if (p.dx == DX_TC) {
         // one pass: activation derivative, bias gradient, fp32 -> split bf16 NHWC (padded to a 64-multiple of channels).
         // Deterministic mode: the pass writes fp32 g instead of adding db, and db is summed from g in a fixed order below.
-        gsplit = (__nv_bfloat16 *)ws.take((size_t)B * gC * Ho * Wo * 4);
-        ESR_REQUIRE(ws.off <= ws.cap, "conv2d_backward: workspace too small");
         const int tpb = split_tiles_per_block(Ho * Wo, gC / 64, B), tiles = (Ho * Wo + 31) / 32;
         k_to_split<true><<<dim3((tiles + tpb - 1) / tpb, gC / 64, B), 256, 0, st>>>(dy, y, act, Cout, gC, Ho * Wo, tpb, gsplit,
-                                                                                   (size_t)B * Ho * Wo * gC, want_dw && !det ? db : nullptr,
-                                                                                   tc_dw && !(det && want_dw) ? nullptr : g);
+                                                                                   (size_t)B * Ho * Wo * gC, want_dw && !p.det ? db : nullptr,
+                                                                                   p.tc_dw && !bias_part ? nullptr : g);
         ESR_LAUNCH_CHECK();
-        if (det && want_dw && (rc = bias_grad(g, B, Cout, Ho * Wo, db, bias_part, st))) return rc;
+        if (bias_part && (rc = bias_grad(g, B, Cout, Ho * Wo, db, bias_part, st))) return rc;
     } else {
-        ESR_REQUIRE(ws.off <= ws.cap, "conv2d_backward: workspace too small");
         if (act == ACT_NONE) {
             ESR_CUDA_CHECK(cudaMemcpyAsync(g, dy, ng * 4, cudaMemcpyDeviceToDevice, st));
         } else {
@@ -1063,59 +1092,44 @@ int esr_conv2d_backward_ex(const float *x, const void *x_split, const float *w, 
         if (want_dw && (rc = bias_grad(g, B, Cout, Ho * Wo, db, bias_part, st))) return rc;
     }
     // ---- dw
-    bool dw_done = !want_dw;
-    if (want_dw && tc_dw) {
+    if (want_dw && p.tc_dw) {
         const __nv_bfloat16 *xsplit = (const __nv_bfloat16 *)x_split;       // saved by the forward, or converted here
         if (!xsplit) {
-            Bump ws2 = ws;                                           // dead after the kernel: dx reuses the space
-            __nv_bfloat16 *xs_ = (__nv_bfloat16 *)ws2.take((size_t)B * Cin * H * W * 4);
-            ESR_REQUIRE(ws2.off <= ws2.cap, "conv2d_backward: workspace too small");
-            if ((rc = split_from_nchw_pad(x, B, Cin, Cin, H * W, xs_, st))) return rc;
-            xsplit = xs_;
+            __nv_bfloat16 *xs = (__nv_bfloat16 *)(ws + L.x_split);
+            if ((rc = split_from_nchw_pad(x, B, Cin, Cin, H * W, xs, st))) return rc;
+            xsplit = xs;
         }
         if ((rc = wgrad_tc(xsplit, gsplit, B, Cin, H, W, Cout, gC, ksz, dw, dw_part, st))) return rc;
-        dw_done = true;
+    } else if (want_dw) {
+        rc = ksz == 3 ? launch_dw<3>(x, g, dw, dw_part, B, Cin, H, W, Cout, Ho, Wo, stride, st)
+                      : launch_dw<1>(x, g, dw, dw_part, B, Cin, H, W, Cout, Ho, Wo, stride, st);
+        if (rc) return rc;
     }
-    if (!dw_done && (rc = generic(2, ksz, x, nullptr, nullptr, g, dw, B, Cin, H, W, Cout, Ho, Wo, stride, 0, st, dw_part))) return rc;
     // ---- dx
-    if (dx) {
-        if (tcd) {
-            float *wt = (float *)ws.take((size_t)gC * Cin * ksz * ksz * 4);
-            void *wp = ws.take(tc_packed_weight_bytes(Cin, gC, ksz * ksz));
-            float *bp = (float *)ws.take(256 * 4);
-            ESR_REQUIRE(ws.off <= ws.cap, "conv2d_backward: workspace too small (%zu > %zu)", ws.off, ws.cap);
-            if (gC != Cout) ESR_CUDA_CHECK(cudaMemsetAsync(wt, 0, (size_t)gC * Cin * ksz * ksz * 4, st));
-            k_weight_rot_t<<<(Cout * Cin * ksz * ksz + 255) / 256, 256, 0, st>>>(w, Cout, gC, Cin, ksz * ksz, wt);
-            ESR_LAUNCH_CHECK();
-            if ((rc = pack_conv_weight(wt, Cin, gC, ksz, wp, st))) return rc;
-            ESR_CUDA_CHECK(cudaMemsetAsync(bp, 0, 256 * 4, st));
-            SplitTensor gsrc; gsrc.base = gsplit; gsrc.n_img = B; gsrc.H = Ho; gsrc.W = Wo; gsrc.C = gC;
-            ConvTCDesc d;
-            d.src[0] = gsrc; d.n_src = 1; d.ntaps = ksz * ksz; d.cout = Cin; d.wpacked = wp; d.bias = bp; d.n_img = B; d.act = ACT_NONE;
-            d.out_f32 = dx; d.out_f32_C = Cin; d.out_f32_nchw = 1;
-            ConvTCArgs a;
-            if ((rc = conv_tc_prepare(d, &a))) return rc;
-            if ((rc = conv_tc_launch(a, st))) return rc;
-        } else if (ksz == 3 && stride == 1 && getenv("ESR_TRAIN_NO_MMA") == nullptr &&
-                   [&] {   // dx = conv(g, rot180(w)^T) on the warp-level tensor cores when the shape is instantiated
-                       Bump w2 = ws;
-                       void *img = w2.take(mma_weight_bytes(Cin, Cout));
-                       if (w2.off > w2.cap) return false;
-                       if (pack_mma_weight_dx(w, Cout, Cin, img, st)) return false;
-                       return conv_mma_nchw(g, img, nullptr, B, Cout, H, W, Cin, 1, ACT_NONE, dx, st) == ESR_OK;
-                   }()) {
-        } else if (ksz == 3 && stride == 1) {
-            // dx = conv(g, rot180(w)^T): the register-tiled forward kernel with the roles of Cin and Cout swapped
-            float *wt = (float *)ws.take((size_t)Cout * Cin * 9 * 4);
-            ESR_REQUIRE(ws.off <= ws.cap, "conv2d_backward: workspace too small (%zu > %zu)", ws.off, ws.cap);
-            k_weight_rot_t<<<(Cout * Cin * 9 + 255) / 256, 256, 0, st>>>(w, Cout, Cout, Cin, 9, wt);
-            ESR_LAUNCH_CHECK();
-            if ((rc = generic(0, 3, g, wt, nullptr, nullptr, dx, B, Cout, H, W, Cin, H, W, 1, ACT_NONE, st))) return rc;
-        } else {
-            if ((rc = generic(1, ksz, nullptr, w, nullptr, g, dx, B, Cin, H, W, Cout, Ho, Wo, stride, 0, st))) return rc;
-        }
+    if (!dx) return ESR_OK;
+    if (p.dx == DX_TC) {
+        float *wt = (float *)(ws + L.wt), *bp = (float *)(ws + L.bias);
+        if (gC != Cout) ESR_CUDA_CHECK(cudaMemsetAsync(wt, 0, (size_t)gC * Cin * ksz * ksz * 4, st));
+        k_weight_rot_t<<<(Cout * Cin * ksz * ksz + 255) / 256, 256, 0, st>>>(w, Cout, gC, Cin, ksz * ksz, wt);
+        ESR_LAUNCH_CHECK();
+        if ((rc = pack_conv_weight(wt, Cin, gC, ksz, ws + L.w_tc, st))) return rc;
+        ESR_CUDA_CHECK(cudaMemsetAsync(bp, 0, 256 * 4, st));
+        SplitTensor gsrc; gsrc.base = gsplit; gsrc.n_img = B; gsrc.H = Ho; gsrc.W = Wo; gsrc.C = gC;
+        return conv_tc_to_nchw(gsrc, ksz * ksz, Cin, ws + L.w_tc, bp, ACT_NONE, dx, st);
     }
-    return ESR_OK;
+    if (p.dx == DX_MMA) {                                             // dx = conv(g, rot180(w)^T) on the warp-level tensor cores
+        if ((rc = pack_mma_weight_dx(w, Cout, Cin, ws + L.w_mma, st))) return rc;
+        return conv_mma_nchw(g, ws + L.w_mma, nullptr, B, Cout, H, W, Cin, 1, ACT_NONE, dx, st);
+    }
+    if (p.dx == DX_R) {
+        // dx = conv(g, rot180(w)^T): the register-tiled forward kernel with the roles of Cin and Cout swapped
+        float *wt = (float *)(ws + L.wt);
+        k_weight_rot_t<<<(Cout * Cin * 9 + 255) / 256, 256, 0, st>>>(w, Cout, Cout, Cin, 9, wt);
+        ESR_LAUNCH_CHECK();
+        return launch_fwd<3>(FWD_R, g, wt, nullptr, dx, B, Cout, H, W, Cin, H, W, 1, ACT_NONE, st);
+    }
+    return ksz == 3 ? launch_dx<3>(p.dx, g, w, dx, B, Cin, H, W, Cout, Ho, Wo, stride, st)
+                    : launch_dx<1>(p.dx, g, w, dx, B, Cin, H, W, Cout, Ho, Wo, stride, st);
 }
 
 int esr_upsample2x_forward(const float *x, int planes, int H, int W, float *y, esr_stream_t stream)

@@ -358,7 +358,7 @@ int esr_dcn_v2_forward(const float *input, const float *weight, const float *bia
  * act: 0 none, 1 relu, 2 sigmoid, 3 tanh (fused into the forward; backward multiplies dy by act'(y)).
  * backward: dx may be NULL (first layer); dw [Cout,Cin,k,k] and db [Cout] are overwritten (not accumulated); dw == db ==
  * NULL computes dx only (a caller that batches the weight gradient of a weight-shared layer, e.g. the ConvGRU steps).
- * workspace: esr_conv2d_workspace_bytes() bytes of device memory owned by the caller.
+ * workspace: esr_conv2d_workspace_bytes() bytes of device memory owned by the caller; a NULL or shorter one is refused (ESR_EINVAL).
  * --------------------------------------------------------------------------------------------- */
 size_t esr_conv2d_workspace_bytes(int B, int Cin, int H, int W, int Cout, int ksz, int stride);
 /* x_split (optional): layers whose forward, dx and dw all run on the tensor cores convert x to the split-bf16 NHWC operand

@@ -14,8 +14,11 @@ TOL is about 4x the error measured on an H100 (DESIGN.md 3 lists the measurement
 
 The training part runs train.conv2d at every narrow (Cin, Cout, stride, act) of the network, at cfg2's training counts and
 at ragged sizes, and checks y, dx, dw and db against float64 the same way (degraded: a lost cross term for the mma.sync /
-wgmma kernels, bf16-rounded x or g for the fp32 FFMA kernels).  It restates the dispatch rule of esr_conv2d_forward /
-backward and asserts that each case lands on the kernels it claims, and that together they cover every branch.
+wgmma kernels, bf16-rounded x or g for the fp32 FFMA kernels).  train_branches restates the rule (conv2d_paths of
+train_ops.cu) that picks the forward, dx and dw kernels; a CPU test asserts that the cases cover every branch, and a GPU test
+profiles the ragged cases and three wide layers, in default and deterministic mode, and asserts that the kernels launched
+are exactly the ones train_branches names.  Another asserts that a workspace one byte short of the reported size is refused
+before anything is launched.
 
 The last part runs forward_sequence and one training window in subprocesses under the process-wide switches
 (ESR_DIRECT_FFMA, ESR_DCN_COLUMNS, ESR_TRAIN_NO_MMA), which are read once per process.
@@ -383,11 +386,12 @@ def tc_dgrad_ok(cin, cout, k, s):
     return s == 1 and 32 <= cout <= 256 and cin <= 256
 
 
-def train_branches(cin, cout, k, s, act):
-    """(forward, dx, dw) kernels esr_conv2d_forward / esr_conv2d_backward launch for this layer."""
+def train_branches(cin, cout, k, s, act, no_mma=False):
+    """(forward, dx, dw) kernels esr_conv2d_forward / esr_conv2d_backward launch for this layer (no_mma: under
+    ESR_TRAIN_NO_MMA)."""
     if tc_fwd_ok(cin, cout, k, s):
         fwd = "k_conv_tc"
-    elif k == 3 and (cin, cout, s) in MMA_CASES and act != "tanh":
+    elif k == 3 and (cin, cout, s) in MMA_CASES and act != "tanh" and not no_mma:
         fwd = "k_conv_mma"
     else:
         fwd = "k_conv_fwd_r" if k == 3 and s == 1 else f"k_conv_fwd_g<{k}>"
@@ -395,7 +399,7 @@ def train_branches(cin, cout, k, s, act):
     if tcd:
         dx = "k_conv_tc"
     elif k == 3 and s == 1:
-        dx = "k_conv_mma" if (cout, cin, 1) in MMA_CASES else "k_conv_fwd_r"
+        dx = "k_conv_mma" if (cout, cin, 1) in MMA_CASES and not no_mma else "k_conv_fwd_r"
     else:
         dx = "k_conv_dgrad_s2" if k == 3 else f"k_conv_dgrad_g<{k}>"
     if tcd and cin % 64 == 0:
@@ -532,6 +536,149 @@ def test_train_narrow_conv2d_vs_fp64(dev, name):
     check(f"{name}.dx", k_dx, dx_got[sel], dx64, dx_deg, dx_is, tol=TRAIN_TOL[k_dx])
     check(f"{name}.dw", k_dw, dw_got, dw64, dw_deg, dw_is, tol=TRAIN_TOL[k_dw])
     check(f"{name}.db", "db", db_got, g64.sum((0, 2, 3)), None, tol=TRAIN_TOL["db"])
+
+
+# ------------------------------------------------------------------------------------------------------------------
+# the kernels train_branches names are the ones that run
+# ------------------------------------------------------------------------------------------------------------------
+CONV_KERNELS = {"k_conv_tc", "k_conv_mma", "k_conv_fwd_r", "k_conv_fwd_g", "k_conv_dgrad_s2", "k_conv_dgrad_g", "k_wgrad_tc",
+                "k_wgrad_tc_det", "k_conv_wgrad_r", "k_conv_wgrad_r_det", "k_conv_wgrad_g", "k_conv_wgrad_g_det", "k_sum_slices"}
+# the ragged cases of TRAIN_NARROW, and small-count versions of three tensor-core layers of test_train_4x_fp64_gpu.CONV4
+# (offset_mask: g padded from 216 to 256 channels): (Cin, Cout, k, stride, act, B, H, W)
+LAUNCH_CASES = {
+    **{n: c[:8] for n, c in TRAIN_NARROW.items() if not n.endswith("_cfg2")},
+    "gru_zr_128_128": (128, 128, 3, 1, "sigmoid", 2, 19, 23),
+    "offset_mask_64_216": (64, 216, 3, 1, None, 2, 13, 21),
+    "global_fusion_128_64_1x1": (128, 64, 1, 1, "relu", 2, 11, 19),
+}
+
+
+def _conv_kernel(name):
+    """Profiler kernel name (demangled or not) -> its name in train_branches, None for kernels outside CONV_KERNELS."""
+    import re
+    m = re.search(r"(?:^|[^a-z_])(k_[a-z0-9_]+)(?:<(\d+)|ILi(\d+)E)?", name)
+    if not m or m.group(1) not in CONV_KERNELS:
+        return None
+    return f"{m.group(1)}<{m.group(2) or m.group(3)}>" if m.group(1).endswith(("_g", "_g_det")) else m.group(1)
+
+
+def expected_kernels(cin, cout, k, s, act, det, no_mma=False):
+    """[forward, backward]: the sorted convolution kernels of one train.conv2d forward and of its backward.  Deterministic
+    mode: dw on its _det kernel, then k_sum_slices (which also sums the bias partials)."""
+    fwd, dx, dw = train_branches(cin, cout, k, s, act, no_mma)
+    if det:
+        dw = dw.replace("<", "_det<") if "<" in dw else dw + "_det"
+    return [[fwd], sorted({dx, dw} | ({"k_sum_slices"} if det else set()))]
+
+
+def profiled_conv_kernels(cin, cout, k, s, act, B, H, W, det):
+    """Runs train.conv2d forward, then backward (dx, dw, db) under torch.profiler (CUDA activity), after one unprofiled run:
+    their kernels as expected_kernels lists them.  A spin kernel between the two marks where the backward starts."""
+    from torch.profiler import ProfilerActivity, profile
+    from esr_b200 import train
+    g = torch.Generator().manual_seed(B * H * W + cin)
+    x = torch.randn(B, cin, H, W, generator=g).cuda().requires_grad_()
+    w = (torch.randn(cout, cin, k, k, generator=g) / math.sqrt(cin * k * k)).cuda().requires_grad_()
+    b = (torch.randn(cout, generator=g) * 0.1).cuda().requires_grad_()
+    Ho, Wo = (H + 2 * (k // 2) - k) // s + 1, (W + 2 * (k // 2) - k) // s + 1
+    dy = torch.randn(B, cout, Ho, Wo, generator=g).cuda()
+    prev = torch.backends.cudnn.deterministic
+    torch.backends.cudnn.deterministic = det
+    try:
+        train.conv2d(x, w, b, s, act).backward(dy)
+        torch.cuda.synchronize()
+        with profile(activities=[ProfilerActivity.CUDA]) as prof:
+            y = train.conv2d(x, w, b, s, act)
+            torch.cuda._sleep(1000)
+            y.backward(dy)
+            torch.cuda.synchronize()
+    finally:
+        torch.backends.cudnn.deterministic = prev
+    names = [e.name for e in sorted(prof.events(), key=lambda e: e.time_range.start)
+             if e.device_type == torch.autograd.DeviceType.CUDA]
+    cut = [i for i, n in enumerate(names) if "spin_kernel" in n]
+    assert len(cut) == 1, names
+    return [sorted({_conv_kernel(n) for n in part} - {None}) for part in (names[:cut[0]], names[cut[0] + 1:])]
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("det", [False, True], ids=["default", "deterministic"])
+@pytest.mark.parametrize("name", list(LAUNCH_CASES))
+def test_train_launches_the_claimed_kernels(dev, name, det):
+    cin, cout, k, s, act, B, H, W = LAUNCH_CASES[name]
+    got = profiled_conv_kernels(cin, cout, k, s, act, B, H, W, det)
+    print(f"[launch] {name} {'deterministic' if det else 'default'}: forward {got[0]}, backward {got[1]}")
+    want = expected_kernels(cin, cout, k, s, act, det)
+    assert got == want, (name, got, want)
+
+
+_LAUNCHES = """
+    import sys, torch
+    from tests.test_small_conv_fp64_gpu import LAUNCH_CASES, profiled_conv_kernels
+    torch.save(profiled_conv_kernels(*LAUNCH_CASES["{name}"], det=False), sys.argv[1])
+"""
+
+
+@pytest.mark.gpu
+def test_train_no_mma_launches_the_claimed_kernels(tmp_path):
+    """Under ESR_TRAIN_NO_MMA the stride-1 dx of a narrow layer runs k_conv_fwd_r on rotated weights: the one row of the
+    rule that default mode does not reach at the network's shapes."""
+    name = "recon1_32_16_21x37"
+    got = _run(_LAUNCHES.format(name=name), tmp_path / "launches.pt", ("ESR_TRAIN_NO_MMA",))
+    want = expected_kernels(*LAUNCH_CASES[name][:5], det=False, no_mma=True)
+    print(f"[launch] {name} ESR_TRAIN_NO_MMA: forward {got[0]}, backward {got[1]}")
+    assert "k_conv_fwd_r" in want[1] and got == want
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("layer", ["tc_64_64", "mma_head_2_8"])
+def test_short_workspace_is_refused(dev, layer):
+    """esr_conv2d_forward and esr_conv2d_backward_ex (default and deterministic) with one byte less workspace than
+    esr_conv2d_workspace_bytes_ex reports, and the mma layer's forward with less than its weight image: each call returns
+    an error and launches nothing, and the outputs keep their sentinel.  With the reported size the same calls run."""
+    from esr_b200 import _lib
+    L, ptr = _lib.lib(), _lib.ptr
+    cin, cout, k, s, act = {"tc_64_64": (64, 64, 3, 1, 1), "mma_head_2_8": (2, 8, 3, 1, 1)}[layer]
+    B, H, W = 2, 13, 21
+    g = torch.Generator(device=dev).manual_seed(7)
+    x, w, b = torch.randn(B, cin, H, W, generator=g, device=dev), torch.randn(cout, cin, k, k, generator=g, device=dev), \
+        torch.randn(cout, generator=g, device=dev)
+    y_in, dy = torch.rand(B, cout, H, W, generator=g, device=dev), torch.randn(B, cout, H, W, generator=g, device=dev)
+    y, dx, dw, db = (torch.full(t.shape, SENTINEL, device=dev) for t in (y_in, x, w, b))
+
+    def forward(ws, n):
+        return L.esr_conv2d_forward(ptr(x), ptr(w), ptr(b), B, cin, H, W, cout, k, s, act, ptr(y), None, ptr(ws), n,
+                                    _lib.stream_ptr())
+
+    def backward(ws, n, flags):
+        return L.esr_conv2d_backward_ex(ptr(x), None, ptr(w), ptr(y_in), ptr(dy), B, cin, H, W, cout, k, s, act, ptr(dx), ptr(dw),
+                                        ptr(db), flags, ptr(ws), n, _lib.stream_ptr())
+    calls = []
+    for flags in (0, _lib.DETERMINISTIC):
+        n = L.esr_conv2d_workspace_bytes_ex(B, cin, H, W, cout, k, s, flags)
+        ws = torch.empty((n,), dtype=torch.uint8, device=dev)
+        calls.append((f"backward flags={flags}", lambda ws=ws, n=n, f=flags: backward(ws, n - 1, f), lambda ws=ws, n=n, f=flags: backward(ws, n, f)))
+        if flags == 0:
+            calls.append(("forward", lambda ws=ws, n=n: forward(ws, n - 1), lambda ws=ws, n=n: forward(ws, n)))
+            if layer == "mma_head_2_8":                    # below the mma weight image (2 x 9 x 8 x 16 bf16 = 4.5 KiB)
+                calls.append(("forward, 256 bytes", lambda ws=ws: forward(ws, 256), None))
+    for what, short, _ in calls:
+        torch.cuda.synchronize()
+        before = L.esr_launch_count()
+        rc = short()
+        torch.cuda.synchronize()
+        assert rc != 0, what
+        assert L.esr_launch_count() == before, what
+        assert "workspace" in L.esr_last_error().decode(), what
+    for t in (y, dx, dw, db):
+        assert bool((t == SENTINEL).all())
+    for what, _, full in calls:                           # the reported size is enough
+        if full is not None:
+            before = L.esr_launch_count()
+            assert full() == 0, what
+            assert L.esr_launch_count() > before, what
+    torch.cuda.synchronize()
+    assert not bool((y == SENTINEL).any()) and not bool((dw == SENTINEL).any())
 
 
 # ------------------------------------------------------------------------------------------------------------------
