@@ -107,6 +107,7 @@ SIGNATURES.update({
                                          c_void_p, c_void_p, c_void_p, c_void_p]),
     "esr_net_get_states": (c_int, [c_void_p, c_void_p, c_void_p]),
     "esr_net_set_states": (c_int, [c_void_p, c_void_p, c_void_p]),
+    "esr_net_copy_states": (c_int, [c_void_p, c_void_p, c_void_p]),
 })
 
 

@@ -674,3 +674,14 @@ extern "C" int esr_net_set_states(esr_net_t net, const float *states, esr_stream
     SplitTensor s0 = view_imgs(n.hs, 0);
     return split_from_nchw_planes(states, 2 * n.B, 64, n.h, n.w, s0.base, n.hs.plane(), (cudaStream_t)stream);
 }
+
+extern "C" int esr_net_copy_states(esr_net_t dst, esr_net_t src, esr_stream_t stream)
+{
+    ESR_REQUIRE(dst && src, "esr_net_copy_states: null net");
+    Net &d = *(Net *)dst, &s = *(Net *)src;
+    ESR_REQUIRE(d.B == s.B && d.h == s.h && d.w == s.w, "esr_net_copy_states: states [%d, 64, %d, %d] and [%d, 64, %d, %d] differ",
+                s.B, s.h, s.w, d.B, d.h, d.w);
+    if (dst == src) return ESR_OK;
+    // slot 0 of both plans: the states at rest, both directions, hi and lo planes, copied as they are
+    return copy_split(view_imgs(s.hs, 0), nullptr, 2 * s.B, view_imgs(d.hs, 0), (cudaStream_t)stream);
+}

@@ -27,6 +27,11 @@ count per shape) with its one host synchronisation, the per-sample lengths from 
 that writes the call's compact segment straight into pinned host memory, and the host-side collection of earlier segments while
 the device runs the next call.  EventStore.write takes whole columns, so a recording's segments stay in host memory until its
 last window has drained; the file is then written on a worker thread.
+
+esr_b200.stream.EventStream gives the same events for a recording that is still arriving, in bounded memory: with mode 'events',
+sliding_window 0, sequence_length = seqn and step_size 1, whatever is pushed in whatever pieces, the concatenation of what it
+returns equals this module's file for the same events byte for byte.  A frame there is final once more than (f + 1) * window
+events have arrived, or when the stream is closed, because of the reference's clamp of a frame's end to num_events - 1.
 """
 import argparse
 import json
@@ -110,6 +115,30 @@ def _segment_views(buf, total):
             buf[:8 * total].view(torch.float64), buf[8 * total:16 * total].view(torch.float64))
 
 
+def emit_call(esr, t0, t1, pinned, collect):
+    """One model call's SR counts esr (CUDA fp32 [n, 2, kH, kW]) -> its compact segment in pinned host memory, on the current
+    stream: the fused cnt2event (or its general chain), collect(False) for earlier calls' segments while the device works,
+    expand_finish (the call's one host synchronisation), plan_segment with the windows' t0 / t1 and one esr_events_to_columns
+    launch.  pinned: the caller's list of idle pinned buffers; one that fits is taken, or a new one made.
+    -> (CUDA event recorded after the launch, buffer, total events, COLUMN_DESC [n])."""
+    ctx = expand_begin(esr, 0, 0)
+    collect(False)                                                  # earlier calls' segments, while the device runs this one
+    rows = expand_finish(ctx, 0)                                    # the call's one host synchronisation
+    desc, total = plan_segment(ctx.ev, t0, t1)
+    fit = next((k for k, b in enumerate(pinned) if b.numel() >= 20 * total), None)
+    if fit is None:                                                 # page-locking costs more than the kernels: reuse across calls
+        pinned.clear()                                              # the idle ones are all too small
+        buf = torch.empty((max(int(25 * total), 1 << 20),), dtype=torch.uint8).pin_memory()
+    else:
+        buf = pinned.pop(fit)
+    if total > 0:
+        desc_d = torch.from_numpy(desc.view(np.uint8)).to(esr.device)
+        events_to_columns(rows.contiguous(), desc_d, int(desc["valid"].max()), *_segment_views(buf, total))
+    done = torch.cuda.Event()
+    done.record()
+    return done, buf, total, desc
+
+
 def _write(path, pieces, hr):
     pieces.sort(key=lambda p: p[0])                                # ascending first window
     cols = [[], [], [], []]
@@ -169,12 +198,9 @@ def super_resolve_recordings(model, stores, dataset_config, out_paths, batch=4, 
                     esr = st["esr"]
                     if tuple(esr.shape[-2:]) != tuple(hr):
                         raise _lib.ESRError(f"superresolve: the model's output {tuple(esr.shape[-2:])} is not the HR resolution {tuple(hr)}")
-                    ctx = expand_begin(esr, 0, 0)
-                    collect(False)                                  # earlier calls' segments, while the device runs this one
-                    rows = expand_finish(ctx, 0)                    # the call's one host synchronisation
                     rs = [members[r] for r in st["rec"]]
-                    desc, total = plan_segment(ctx.ev, [times[r][0][w] for r, w in zip(rs, st["win"])],
-                                               [times[r][1][w] for r, w in zip(rs, st["win"])])
+                    done, buf, total, desc = emit_call(esr, [times[r][0][w] for r, w in zip(rs, st["win"])],
+                                                       [times[r][1][w] for r, w in zip(rs, st["win"])], pinned, collect)
                     runs = []                                       # a recording's windows of one call are consecutive samples
                     for j, (r, w) in enumerate(zip(rs, st["win"])):
                         counts[r][w] = desc["valid"][j]
@@ -184,17 +210,6 @@ def super_resolve_recordings(model, stores, dataset_config, out_paths, batch=4, 
                             runs[-1][4] = a + int(desc["valid"][j])
                         else:
                             runs.append([r, w, 1, a, a + int(desc["valid"][j])])
-                    fit = next((k for k, b in enumerate(pinned) if b.numel() >= 20 * total), None)
-                    if fit is None:                                 # page-locking costs more than the kernels: reuse across calls
-                        pinned.clear()                              # the idle ones are all too small
-                        buf =torch.empty((max(int(25 * total), 1 << 20),), dtype=torch.uint8).pin_memory()
-                    else:
-                        buf = pinned.pop(fit)
-                    if total > 0:
-                        desc_d = torch.from_numpy(desc.view(np.uint8)).to(dev)
-                        events_to_columns(rows.contiguous(), desc_d, int(desc["valid"].max()), *_segment_views(buf, total))
-                    done = torch.cuda.Event()
-                    done.record()
                     pending.append((done, buf, total, runs))
         collect(True)
         for j in jobs:

@@ -306,6 +306,10 @@ int esr_net_forward_profiled(esr_net_t net, const float *input, const int32_t *i
 /* states: fp32 [2,B,64,H/8,W/8] (forward-direction state, reverse-direction state), the reference's self.states */
 int esr_net_get_states(esr_net_t net, float *states, esr_stream_t stream);
 int esr_net_set_states(esr_net_t net, const float *states, esr_stream_t stream);
+/* Copy src's carried states into dst bit for bit (both directions, both split planes; no fp32 round trip) with one launch on
+ * `stream`.  The plans must have the same B, H and W; they may differ in L.  esr_b200.stream hands the state from one
+ * forward_sequence length to the next this way. */
+int esr_net_copy_states(esr_net_t dst, esr_net_t src, esr_stream_t stream);
 
 /* ---------------------------------------------------------------------------------------------
  * The `_ext.dcn_v2_forward` operator (modulated deformable convolution), reference layouts in and out.
