@@ -107,7 +107,9 @@ SIGNATURES.update({
                                          c_void_p, c_void_p, c_void_p, c_void_p]),
     "esr_net_get_states": (c_int, [c_void_p, c_void_p, c_void_p]),
     "esr_net_set_states": (c_int, [c_void_p, c_void_p, c_void_p]),
-    "esr_net_copy_states": (c_int, [c_void_p, c_void_p, c_void_p]),
+    "esr_net_state_bytes": (c_size_t, [c_int, c_int]),
+    "esr_net_gather_states": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p]),
+    "esr_net_scatter_states": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p]),
 })
 
 
@@ -117,6 +119,7 @@ SIGNATURES.update({
                                   c_void_p, c_void_p, c_void_p]),
     "esr_gather_events_aug": (c_int, [c_void_p] * 7 + [c_int, c_int, c_int, c_i64] + [c_void_p] * 5),
     "esr_encode_frames_multi": (c_int, [c_void_p, c_void_p, c_int, c_i64] + [c_int] * 4 + [c_void_p] * 3),
+    "esr_events_append_rings": (c_int, [c_void_p, c_int, c_i64] + [c_void_p] * 4),
     "esr_metrics_workspace_bytes": (c_size_t, [c_int, c_int, c_int, c_int]),
     "esr_metrics_planes": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, ctypes.c_double, c_void_p, c_void_p, c_size_t, c_void_p]),
     "esr_lpips_param_bytes": (c_size_t, []),

@@ -675,13 +675,59 @@ extern "C" int esr_net_set_states(esr_net_t net, const float *states, esr_stream
     return split_from_nchw_planes(states, 2 * n.B, 64, n.h, n.w, s0.base, n.hs.plane(), (cudaStream_t)stream);
 }
 
-extern "C" int esr_net_copy_states(esr_net_t dst, esr_net_t src, esr_stream_t stream)
+// ---- state rows: one sample's carried state outside any plan -----------------------------------------------------------
+// Row layout (private to this file): [direction 2][plane 2][h][w][64] bf16 -- forward then reverse direction, hi then lo
+// split plane, each an image of slot 0 as the plan keeps it, so a row moves in and out of a plan as raw bf16 words.
+static size_t state_img8(int H, int W) { return (size_t)((H + 7) / 8) * ((W + 7) / 8) * 64 / 8; }
+
+extern "C" size_t esr_net_state_bytes(int H, int W)
 {
-    ESR_REQUIRE(dst && src, "esr_net_copy_states: null net");
-    Net &d = *(Net *)dst, &s = *(Net *)src;
-    ESR_REQUIRE(d.B == s.B && d.h == s.h && d.w == s.w, "esr_net_copy_states: states [%d, 64, %d, %d] and [%d, 64, %d, %d] differ",
-                s.B, s.h, s.w, d.B, d.h, d.w);
-    if (dst == src) return ESR_OK;
-    // slot 0 of both plans: the states at rest, both directions, hi and lo planes, copied as they are
-    return copy_split(view_imgs(s.hs, 0), nullptr, 2 * s.B, view_imgs(d.hs, 0), (cudaStream_t)stream);
+    return H > 0 && W > 0 ? 4 * state_img8(H, W) * 8 * sizeof(__nv_bfloat16) : 0;
+}
+
+namespace esr {
+// one thread per 16 bytes: i -> (slot b, part k = direction * 2 + plane, element e); consecutive threads, consecutive e
+template <bool GATHER>
+__global__ void __launch_bounds__(256)
+k_state_rows(__nv_bfloat16 *__restrict__ slot0, size_t plane, int B, size_t img8, uint4 *__restrict__ pool,
+             const int32_t *__restrict__ row_of_slot)
+{
+    const size_t total = (size_t)B * 4 * img8;
+    for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
+        const int b = (int)(i / (4 * img8));
+        const size_t r = i % (4 * img8), k = r / img8, e = r % img8;
+        const int row = row_of_slot[b];
+        uint4 *s = reinterpret_cast<uint4 *>(slot0 + (k & 1) * plane) + ((k >> 1) * B + b) * img8 + e;
+        if (GATHER)
+            *s = row < 0 ? make_uint4(0, 0, 0, 0) : pool[(size_t)row * 4 * img8 + r];
+        else if (row >= 0)
+            pool[(size_t)row * 4 * img8 + r] = *s;
+    }
+}
+} // namespace esr
+
+static int state_rows(esr_net_t net, void *pool, const int32_t *row_of_slot, bool gather, esr_stream_t stream)
+{
+    ESR_REQUIRE(net && pool && row_of_slot, "esr_net_%s_states: null pointer", gather ? "gather" : "scatter");
+    Net &n = *(Net *)net;
+    ESR_REQUIRE(((uintptr_t)pool & 15) == 0, "esr_net_%s_states: the pool must be 16-byte aligned", gather ? "gather" : "scatter");
+    const size_t img8 = state_img8(n.H, n.W), total = (size_t)n.B * 4 * img8;
+    const unsigned grid = (unsigned)std::min<int64_t>(ceil_div64((int64_t)total, 256), (int64_t)dev_info().sm_count * 16);
+    __nv_bfloat16 *s0 = view_imgs(n.hs, 0).base;
+    if (gather)
+        k_state_rows<true><<<grid, 256, 0, (cudaStream_t)stream>>>(s0, n.hs.plane(), n.B, img8, (uint4 *)pool, row_of_slot);
+    else
+        k_state_rows<false><<<grid, 256, 0, (cudaStream_t)stream>>>(s0, n.hs.plane(), n.B, img8, (uint4 *)pool, row_of_slot);
+    ESR_LAUNCH_CHECK();
+    return ESR_OK;
+}
+
+extern "C" int esr_net_gather_states(esr_net_t net, const void *pool, const int32_t *row_of_slot, esr_stream_t stream)
+{
+    return state_rows(net, const_cast<void *>(pool), row_of_slot, true, stream);
+}
+
+extern "C" int esr_net_scatter_states(esr_net_t net, void *pool, const int32_t *row_of_slot, esr_stream_t stream)
+{
+    return state_rows(net, pool, row_of_slot, false, stream);
 }

@@ -127,11 +127,55 @@ k_encode_frames_multi(const unsigned long long *__restrict__ cols, const FrameDe
     }
 }
 
+// ---------------------------------------------------------------------------------------------------------------------
+// Many live streams' new events -> their HBM rings in one launch (esr_b200.stream.EventStreamPool).  Segment d = rows
+// [src, src + count) of the packed source columns goes to ring positions position, position + 1, ... mod capacity.
+struct RingDesc {
+    unsigned long long xs, ys, ps;     // the ring's columns: int16, int16, float64
+    long long capacity, position, count, src;
+};
+
+// grid (blocks per segment, segments), both with stride loops; consecutive threads write consecutive ring elements
+__global__ void __launch_bounds__(256)
+k_append_rings(const RingDesc *__restrict__ desc, int n_desc, const short *__restrict__ src_xs, const short *__restrict__ src_ys,
+               const double *__restrict__ src_ps)
+{
+    for (int s = blockIdx.y; s < n_desc; s += gridDim.y) {
+        const RingDesc d = desc[s];
+        if (d.capacity <= 0) continue;
+        const long long n = min(max(d.count, 0LL), d.capacity), p0 = d.position % d.capacity;
+        short *xs = reinterpret_cast<short *>(d.xs), *ys = reinterpret_cast<short *>(d.ys);
+        double *ps = reinterpret_cast<double *>(d.ps);
+        for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
+            long long j = p0 + i;
+            if (j >= d.capacity) j -= d.capacity;                  // the wrap: n <= capacity
+            xs[j] = src_xs[d.src + i];
+            ys[j] = src_ys[d.src + i];
+            ps[j] = src_ps[d.src + i];
+        }
+    }
+}
+
 } // namespace esr
 
 using namespace esr;
 
 static_assert(sizeof(FrameDesc) == sizeof(esr_frame_desc), "esr_frame_desc layout");
+static_assert(sizeof(RingDesc) == sizeof(esr_ring_desc), "esr_ring_desc layout");
+
+extern "C" int esr_events_append_rings(const esr_ring_desc *desc, int n_desc, int64_t max_count, const int16_t *src_xs,
+                                       const int16_t *src_ys, const double *src_ps, esr_stream_t stream)
+{
+    ESR_REQUIRE(n_desc >= 0 && max_count >= 0, "esr_events_append_rings: negative count");
+    if (n_desc == 0 || max_count == 0) return ESR_OK;
+    ESR_REQUIRE(desc && src_xs && src_ys && src_ps, "esr_events_append_rings: null pointer");
+    // ~4 events per thread for the longest segment, capped; segments on grid y
+    const int64_t bx = max((int64_t)1, min(ceil_div64(max_count, 256 * 4), (int64_t)dev_info().sm_count * 16));
+    const dim3 grid((unsigned)bx, (unsigned)min(n_desc, 65535));
+    k_append_rings<<<grid, 256, 0, (cudaStream_t)stream>>>(reinterpret_cast<const RingDesc *>(desc), n_desc, src_xs, src_ys, src_ps);
+    ESR_LAUNCH_CHECK();
+    return ESR_OK;
+}
 
 extern "C" int esr_encode_frames_multi(const uint64_t *cols, const esr_frame_desc *desc, int n_frames, int64_t max_len, int H, int W,
                                        int kH, int kW, float *out_cnt, float *out_scaled_cnt, esr_stream_t stream)

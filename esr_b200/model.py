@@ -214,14 +214,6 @@ class DeepRecurrNet(nn.Module):
                         continue
                     _lib.check(_lib.lib().esr_net_reset_sample_states(p.handle, b, _lib.stream_ptr()), "esr_net_reset_sample_states")
 
-    def carry_states(self, src, dst, device):
-        """Copy the carried ConvGRU states of the inference plan of shape src = (B, L, H, W) into the plan of shape dst (same
-        B, H, W, another L; made when missing), bit for bit: a forward_sequence call of length dst then continues the
-        recurrence that the calls of length src left."""
-        with torch.cuda.device(device):
-            a, b = self._plans[tuple(src)], self._plan(*dst, device)
-            _lib.check(_lib.lib().esr_net_copy_states(b.handle, a.handle, _lib.stream_ptr()), "esr_net_copy_states")
-
     def states(self, B, L, H, W):
         """The carried states [h_fwd, h_rev] (each Bx64xhxw) of the plan for this shape -- the reference's
         `time_propagate.states`."""

@@ -88,15 +88,17 @@ def middle_frame_times(event_indices, ts, mids):
     return t0, t1
 
 
-def plan_segment(ev, t0, t1):
+def plan_segment(ev, t0, t1, order=None):
     """Descriptors of one model call: sample j's ev[j] events go to rows [dst[j], dst[j] + ev[j]) of the call's segment, samples
-    in order.  -> (COLUMN_DESC [n], total events)."""
+    in order -- or in the order of the sample indices `order`, where samples left out are not written (valid 0).
+    -> (COLUMN_DESC [n], total events)."""
     ev = np.asarray(ev, np.int64)
     desc = np.zeros(len(ev), COLUMN_DESC)
-    desc["valid"] = ev
-    desc["dst"] = np.cumsum(ev) - ev
     desc["t0"], desc["t1"] = t0, t1
-    return desc, int(ev.sum())
+    order = np.arange(len(ev)) if order is None else np.asarray(order, np.int64)
+    desc["valid"][order] = ev[order]
+    desc["dst"][order] = np.cumsum(ev[order]) - ev[order]
+    return desc, int(ev[order].sum())
 
 
 def events_to_columns(rows, desc, max_valid, xs, ys, ts, ps):
@@ -115,16 +117,16 @@ def _segment_views(buf, total):
             buf[:8 * total].view(torch.float64), buf[8 * total:16 * total].view(torch.float64))
 
 
-def emit_call(esr, t0, t1, pinned, collect):
+def emit_call(esr, t0, t1, pinned, collect, order=None):
     """One model call's SR counts esr (CUDA fp32 [n, 2, kH, kW]) -> its compact segment in pinned host memory, on the current
     stream: the fused cnt2event (or its general chain), collect(False) for earlier calls' segments while the device works,
-    expand_finish (the call's one host synchronisation), plan_segment with the windows' t0 / t1 and one esr_events_to_columns
-    launch.  pinned: the caller's list of idle pinned buffers; one that fits is taken, or a new one made.
+    expand_finish (the call's one host synchronisation), plan_segment with the windows' t0 / t1 (and the sample `order`) and
+    one esr_events_to_columns launch.  pinned: the caller's list of idle pinned buffers; one that fits is taken, or a new one made.
     -> (CUDA event recorded after the launch, buffer, total events, COLUMN_DESC [n])."""
     ctx = expand_begin(esr, 0, 0)
     collect(False)                                                  # earlier calls' segments, while the device runs this one
     rows = expand_finish(ctx, 0)                                    # the call's one host synchronisation
-    desc, total = plan_segment(ctx.ev, t0, t1)
+    desc, total = plan_segment(ctx.ev, t0, t1, order)
     fit = next((k for k, b in enumerate(pinned) if b.numel() >= 20 * total), None)
     if fit is None:                                                 # page-locking costs more than the kernels: reuse across calls
         pinned.clear()                                              # the idle ones are all too small

@@ -306,10 +306,18 @@ int esr_net_forward_profiled(esr_net_t net, const float *input, const int32_t *i
 /* states: fp32 [2,B,64,H/8,W/8] (forward-direction state, reverse-direction state), the reference's self.states */
 int esr_net_get_states(esr_net_t net, float *states, esr_stream_t stream);
 int esr_net_set_states(esr_net_t net, const float *states, esr_stream_t stream);
-/* Copy src's carried states into dst bit for bit (both directions, both split planes; no fp32 round trip) with one launch on
- * `stream`.  The plans must have the same B, H and W; they may differ in L.  esr_b200.stream hands the state from one
- * forward_sequence length to the next this way. */
-int esr_net_copy_states(esr_net_t dst, esr_net_t src, esr_stream_t stream);
+/* State rows: the carried ConvGRU state of one sample kept outside any plan, so that many independent streams can share the
+ * plans' batch slots (esr_b200.stream.EventStreamPool).  A row holds both directions and both split-bf16 planes in a layout
+ * private to the library, esr_net_state_bytes(H, W) bytes for a net of input size H x W (0 for a non-positive size); a pool
+ * is an array of rows, 16-byte aligned.  row_of_slot: device int32 [B] (B of the net).
+ *   gather : sample b's state (slot 0, images b and B + b, both planes) := pool row row_of_slot[b]; row -1 gives zeros, a new
+ *            stream's state.  Rows may repeat.
+ *   scatter: pool row row_of_slot[b] := sample b's state; row -1 is skipped.  Rows other than -1 must not repeat.
+ * Bit-exact copies (no fp32 round trip); one launch each on `stream`, no allocation, no host synchronisation:
+ * graph-capturable.  The plans' own states need no reset when every call is framed by a gather and a scatter. */
+size_t esr_net_state_bytes(int H, int W);
+int esr_net_gather_states(esr_net_t net, const void *pool, const int32_t *row_of_slot, esr_stream_t stream);
+int esr_net_scatter_states(esr_net_t net, void *pool, const int32_t *row_of_slot, esr_stream_t stream);
 
 /* ---------------------------------------------------------------------------------------------
  * The `_ext.dcn_v2_forward` operator (modulated deformable convolution), reference layouts in and out.
@@ -504,6 +512,19 @@ typedef struct {
 } esr_frame_desc;
 int esr_encode_frames_multi(const uint64_t *cols, const esr_frame_desc *desc, int n_frames, int64_t max_len, int H, int W, int kH,
                             int kW, float *out_cnt, float *out_scaled_cnt, esr_stream_t stream);
+
+/* New events of many live streams -> each stream's ring, in one launch (esr_b200.stream.EventStreamPool uploads a round
+ * this way).  desc: device table [n_desc], one segment per stream: rows [src, src + count) of the source columns src_xs,
+ * src_ys (int16) and src_ps (float64) go to ring elements (position + i) mod capacity of the ring columns xs, ys, ps (device
+ * addresses; position is the stream's event count before the segment).  0 <= count <= capacity and capacity > 0; rings must
+ * not overlap.  The source may be pinned host memory or device memory.  max_count: the largest count (grid sizing).
+ * No allocation, no synchronisation: graph-capturable. */
+typedef struct {
+    uint64_t xs, ys, ps;
+    int64_t capacity, position, count, src;
+} esr_ring_desc;
+int esr_events_append_rings(const esr_ring_desc *desc, int n_desc, int64_t max_count, const int16_t *src_xs,
+                            const int16_t *src_ys, const double *src_ps, esr_stream_t stream);
 
 /* ---------------------------------------------------------------------------------------------
  * Padded cnt2event rows -> the columns of an event file (esr_b200/superresolve.py).  Completes
